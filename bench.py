@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench.py — build_octree (+ frustum query, X-ray tiles) throughput on B200, one JSON line on rank 0.
+"""bench.py — build_octree (+ frustum query, X-ray tiles) throughput on H100, one JSON line on rank 0.
 
   python bench.py --gpus N --steps K --warmup W          the CUDA path (this repo)
   python bench.py --impl reference --gpus N ...           the reference's CPU algorithm (oracle port) on the host cores
 
 A step = one build_octree over one batch of synthetic points (BASELINE.json config 2: Gaussian clusters in a 1024 m cube,
-resolution 1024/2^20 -> depth 20, 1e9 points per GPU).  At N > 1 every rank owns the same number of points of one global index
-space (weak scaling; config 4 = 8e9 points on 8 GPUs): the points shard by level-2 octree prefix and move once to their owners
+resolution 1024/2^20 -> depth 20, 5e8 points per GPU).  At N > 1 every rank owns the same number of points of one global index
+space (weak scaling; config 4 = 4e9 points on 8 GPUs): the points shard by level-2 octree prefix and move once to their owners
 over NVLink (one fused rank + peer-store kernel, CUDA-IPC mapped receive slabs; NCCL carries only the small all-reduces).
 `value` = points / device time of the step (a CUDA event pair around the call, host planning included, max over ranks) with the
 inputs resident in HBM; `e2e` = the same build through the C-ABI host entry point: pinned host buffers -> H2D -> build -> D2H
@@ -42,7 +42,7 @@ def _peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 class ClockSampler:
@@ -397,6 +397,74 @@ def full_size_check(tree, D, torch, dist, world, n, dev):
     return {"ok": got == want, "points": got[0], "expected_points": NT, "sum_idx_ok": got[1] == want[1], "sum_idx_sq_ok": got[2] == want[2]}
 
 
+DUMP_SAMPLE = 1 << 19  # point slots in the --dump-outputs sample
+DUMP_SEED = 20240607
+DUMP_LIMIT = 64 << 20  # bytes of .npy payload at most
+
+
+def dump_sample_index(meta, n, sample=DUMP_SAMPLE, seed=DUMP_SEED):
+    """A fixed, seeded sample of the point slots of an octree with n points and node table `meta`: per slot its node (index
+    into `meta`), bytes per coordinate and the byte offset of its position code in the octree's xyz store."""
+    import numpy as np
+
+    slots = np.sort(np.random.default_rng(seed).choice(n, min(n, sample), replace=False)).astype(np.int64)
+    po = meta["point_offset"].astype(np.int64)
+    order = np.lexsort((meta["num_points"], po))  # among nodes at the same offset the empty ones come first
+    node = order[np.searchsorted(po[order], slots, side="right") - 1]
+    bpc = np.array([0, 1, 2, 4, 8], np.int64)[meta["enc"][node]]
+    byte0 = meta["xyz_byte_offset"][node].astype(np.int64) + (slots - po[node]) * 3 * bpc
+    return slots, node, bpc, byte0
+
+
+def dump_outputs(tree, directory, torch, dev):
+    """--dump-outputs: what a caller of the timed build receives from its last step, as DIR/<name>.npy in float64 / float32.
+    The node table in full (node ids as four 32-bit words, so that float64 holds them exactly); the per-point arrays (source
+    index, colour, position code as stored in its node's encoding) as a fixed seeded sample of DUMP_SAMPLE slots."""
+    import ctypes as C
+
+    import numpy as np
+
+    from point_cloud_viewer_b200 import _native as N
+    from point_cloud_viewer_b200.distributed import _RawCuda
+
+    meta = tree.meta
+    slots, node, bpc, byte0 = dump_sample_index(meta, tree.num_points)
+    p = [C.c_void_p() for _ in range(4)]
+    N.check(N.lib().pcv_octree_device_arrays(tree.h, *[C.byref(v) for v in p]))
+    xyz = torch.as_tensor(_RawCuda(p[0].value, (tree.xyz_bytes,), "|u1"), device=dev)
+    rgb = torch.as_tensor(_RawCuda(p[1].value, (tree.num_points, 3), "|u1"), device=dev)
+    src = torch.as_tensor(_RawCuda(p[3].value, (tree.num_points,), "<i4"), device=dev)  # u32 viewed as i32
+    s = torch.from_numpy(slots).to(dev)
+    idx = torch.clamp(torch.from_numpy(byte0).to(dev)[:, None] + torch.arange(24, device=dev)[None, :], max=tree.xyz_bytes - 1)
+    raw = xyz[idx].cpu().numpy()
+    codes = np.zeros((len(slots), 3), np.float64)
+    enc = meta["enc"][node]
+    for e, dt in ((1, "u1"), (2, "<u2"), (3, "<f4"), (4, "<f8")):
+        sel = enc == e
+        if sel.any():
+            b = np.dtype(dt).itemsize
+            codes[sel] = np.ascontiguousarray(raw[sel, : 3 * b]).view(dt).reshape(-1, 3).astype(np.float64)
+    hi, lo = meta["id_high"], meta["id_low"]
+    out = {
+        "node_id_words": np.stack([hi >> np.uint64(32), hi & np.uint64(0xFFFFFFFF), lo >> np.uint64(32), lo & np.uint64(0xFFFFFFFF)], 1).astype(np.float64),
+        "node_num_points": meta["num_points"].astype(np.float64),
+        "node_level": meta["level"].astype(np.float64),
+        "node_encoding": meta["enc"].astype(np.float64),
+        "node_cube": meta["cube"].astype(np.float64),
+        "node_point_offset": meta["point_offset"].astype(np.float64),
+        "sample_slot": slots.astype(np.float64),
+        "sample_src_index": (src[s].to(torch.int64) & 0xFFFFFFFF).cpu().numpy().astype(np.float64),
+        "sample_rgb": rgb[s].cpu().numpy().astype(np.float32),
+        "sample_xyz_code": codes,
+    }
+    total = sum(a.nbytes for a in out.values())
+    if total > DUMP_LIMIT:
+        raise RuntimeError("--dump-outputs: %d bytes exceed the %d-byte limit" % (total, DUMP_LIMIT))
+    os.makedirs(directory, exist_ok=True)
+    for name, a in out.items():
+        np.save(os.path.join(directory, name + ".npy"), a)
+
+
 def run_ours(args):
     import numpy as np
     import torch
@@ -498,6 +566,8 @@ def run_ours(args):
     value = world * n / (ms_per_step * 1e3)
     stats = ctx.last_build_stats() if world == 1 else last.stats
     nodes = int(last.num_nodes)
+    if args.dump_outputs:
+        dump_outputs(last, args.dump_outputs, torch, dev)
 
     out = {
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_per_step,
@@ -551,14 +621,8 @@ def run_ours(args):
         top = max(ks.items(), key=lambda kv: kv[1]["ms"])
         tname, tst = top
         achieved = tst["algorithmic_bytes"] / (tst["ms"] * 1e-3) / 1e9 if tst["ms"] > 0 else 0.0
-        traffic = None
-        try:  # DRAM bytes per launch from the committed `ncu --set full` capture (ratio to algorithmic bytes at N = 1e8)
-            with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-                traffic = json.load(f)[tname]["ratio"] * tst["algorithmic_bytes"] / max(1, tst["launches"])
-        except Exception:
-            pass
         out["roofline"] = {
-            "bound": "hbm", "kernel": tname, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+            "bound": "hbm", "kernel": tname, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": None,
             "peak_source": peak_src, "launches": tst["launches"], "avg_launch_ms": tst["ms"] / max(1, tst["launches"]),
             "algorithmic_bytes_per_launch": tst["algorithmic_bytes"] / max(1, tst["launches"]),
             "note": "per-kernel bytes are the pass-local reads + writes (records 16 B + colour 4 B + digit 1 B per point and pass); whole_build uses the SURVEY 8(d) compulsory bytes: 27 N + sum over nodes of n (3 bpc + 3)",
@@ -605,7 +669,7 @@ def run_ours(args):
                 t.free()
                 return b
 
-            e2e_step()  # two warm-up calls: the stream-ordered pool grows to hold the 27 GB staging copy
+            e2e_step()  # two warm-up calls: the stream-ordered pool grows to hold the staging copy (27 B per point)
             e2e_step()
             torch.cuda.synchronize()
             w0 = time.perf_counter()
@@ -686,7 +750,7 @@ def run_ours(args):
 
 
 def bench_query(ctx, pcv, torch, O, tree, args, bmin, bmax, peak, cores, res):
-    """Config 3: 1000 random frusta (two far planes) over the resident 1e9-point octree.  Device time from the library's CUDA
+    """Config 3: 1000 random frusta (two far planes) over the resident octree of the timed build.  Device time from the library's CUDA
     events; bytes = B_query of SURVEY 8(d) (decode read of every tested point + 27 B per survivor).  CPU baseline: the oracle's
     ParallelIterator port (cores - 1 threads, point_cloud_client/src/lib.rs:67) over an octree of the first --cpu-points points."""
     G = pcv.geometry
@@ -711,7 +775,7 @@ def bench_query(ctx, pcv, torch, O, tree, args, bmin, bmax, peak, cores, res):
                      "Mpoints_per_s_tested": float(tested.sum()) / (qs["ms_device"] * 1e3), "gpu_launches": int(qs["kernel_launches"]),
                      "roofline": {"bound": "hbm", "kernel": "k_cull", "achieved": gbps, "peak": peak, "unit": "GB/s", "frac": gbps / peak,
                                   "algorithmic_bytes": int(qs["algorithmic_bytes"]), "cull_kernel_ms": qs["ms_cull"]}}
-    # CPU baseline on a sample octree (the oracle cannot hold 1e9 points in this run's time budget)
+    # CPU baseline on a sample octree (the oracle cannot build the full size in this run's time budget)
     nc = int(args.cpu_points)
     cx, cy, cz, crgb = O.synth_points(O.SYNTH_GAUSS_CLUSTERS, SEED, 0, nc, num_threads=cores)
     o = O.build(cx, cy, cz, crgb.reshape(-1, 3), res, bmin, bmax, num_threads=cores)
@@ -776,7 +840,7 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    ap.add_argument("--points", type=float, default=1e9, help="points per GPU per step (the same at every N)")
+    ap.add_argument("--points", type=float, default=5e8, help="points per GPU per step (the same at every N); 5e8 keeps the build's ~106 B per point within an 80 GB H100")
     ap.add_argument("--levels-per-pass", type=int, default=2, help="(accepted for compatibility: the split phase resolves two levels per pass)")
     ap.add_argument("--prefix-levels", type=int, default=2)
     ap.add_argument("--frusta", type=int, default=1000)
@@ -787,7 +851,13 @@ def main():
     ap.add_argument("--ref-points", type=float, default=1e8, help="points of the bounded sample each --impl reference step builds")
     ap.add_argument("--no-extras", action="store_true", help="profiling runs: only the timed build steps (no roofline / query / e2e / CPU legs)")
     ap.add_argument("--roofline-only", action="store_true", help="development runs: timed steps + per-kernel roofline, none of the other legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write the last step's octree (node table + a fixed seeded sample of its points) "
+                    "as DIR/<name>.npy; single GPU, CUDA path")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.impl != "ours" or int(os.environ.get("WORLD_SIZE", "1")) > 1):
+        ap.error("--dump-outputs writes the single-GPU CUDA build's outputs")
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3
     if args.impl == "reference":

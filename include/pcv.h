@@ -1,5 +1,5 @@
 /*
- * pcv.h — C ABI of the B200-native octree builder / LOD + frustum point-query engine.
+ * pcv.h — C ABI of the H100-native octree builder / LOD + frustum point-query engine.
  *
  * This is the drop-in boundary for point_cloud_viewer's hot path: each entry point replaces a Rust
  * function or trait method of crate `point_viewer` (citations = reference file:line).  The reference

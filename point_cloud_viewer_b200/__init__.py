@@ -1,4 +1,4 @@
-"""point_cloud_viewer_b200 — B200-native octree builder + LOD / frustum point-query engine.
+"""point_cloud_viewer_b200 — H100-native octree builder + LOD / frustum point-query engine.
 
 The product is the CUDA shared library behind include/pcv.h (csrc/).  This package is the thin host
 layer used by tests and bench.py: it mirrors the names of the reference's interface for this path
@@ -450,9 +450,9 @@ class Octree:
         return xyz, rgb, inten, src
 
     def free(self):
-        if self.h:
+        if self.h and self.ctx.h:  # the library frees through the context: after Context.close() there is nothing left to call
             N.lib().pcv_octree_free(self.h)
-            self.h = None
+        self.h = None
 
     def __del__(self):
         try:
@@ -649,9 +649,9 @@ class S2Cloud:
         N.check(N.lib().pcv_s2_cells(self.h, _p(self.cell_ids), _p(self.cell_counts)))
 
     def free(self):
-        if self.h:
+        if self.h and self.ctx.h:  # as Octree.free
             N.lib().pcv_s2_free(self.h)
-            self.h = None
+        self.h = None
 
     def write_dir(self, directory):
         """<token>.xyz / .rgb / .intensity per cell + meta.pb, as S2Splitter<RawNodeWriter> leaves them."""

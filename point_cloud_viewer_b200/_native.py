@@ -252,7 +252,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise ImportError(
                 "point_cloud_viewer_b200: %s is missing - build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). There is no CPU fallback." % LIB_PATH
+                "(nvcc, sm_90a). There is no CPU fallback." % LIB_PATH
             )
         L = C.CDLL(LIB_PATH)
         for name, res, args in SYMBOLS:

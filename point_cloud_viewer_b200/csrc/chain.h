@@ -71,7 +71,7 @@ PCV_HD double clamp01(double x) {
 }
 
 // Rust `f64 as u16/u8` as the callers need it (they cap the result at 255 / 65535): truncate toward zero, NaN -> 0,
-// negative -> 0, huge -> saturated.  On the GPU this goes through the SIGNED conversion: measured on sm_100,
+// negative -> 0, huge -> saturated.  On the GPU this goes through the SIGNED conversion:
 // cvt.rzi.u32.f64 returns 0x80000000 for NaN (not 0), while cvt.rzi.s32.f64 gives INT_MIN for NaN / -inf and INT_MAX
 // for +inf / huge, so max(v, 0) has exactly the semantics of the Rust cast below 2^31.
 PCV_HD uint32_t trunc_u32(double s) {

@@ -1,4 +1,4 @@
-// kernels_build.cuh — sm_100a kernels of the octree build and the CUDA Backend that drives them.
+// kernels_build.cuh — sm_90a kernels of the octree build and the CUDA Backend that drives them.
 //
 //   k_bbox      a1  find_bounding_box (generation.rs:256-270): streaming min/max, warp-shuffle reduce
 //   k_ingest    a3-a6  raw position -> first step of the chain (chain.h): level-1 codes + the first pass's digits
@@ -100,8 +100,7 @@ __global__ void __launch_bounds__(256) k_bbox(PointsView p, double* __restrict__
 // ------------------------------------------------------------------------------------------------
 // k_place streams leaf tiles whose addresses are known long before they are needed.  One thread asks the TMA unit to
 // pull the tile that is about one wave of resident blocks away into L2 (cp.async.bulk.prefetch.L2: no registers, no L1
-// lines, no completion to wait for), so that when that block runs its loads hit L2 instead of HBM (measured at N = 1e9:
-// k_place 13.4 -> 11.2 ms; the same prefetch did not help k_hist / k_scatter, whose time is not load latency).  The byte
+// lines, no completion to wait for), so that when that block runs its loads hit L2 instead of HBM.  The byte
 // range is shrunk to 16-byte alignment inside [p, p + bytes): nothing outside the caller's range is ever touched.
 __device__ __forceinline__ void l2_prefetch(const void* p, uint64_t bytes) {
     const uintptr_t b = (reinterpret_cast<uintptr_t>(p) + 15) & ~(uintptr_t)15;
@@ -1567,7 +1566,7 @@ struct CudaBackend : Backend {
             for (int a = 0; a < 3; ++a) mn[a] = mx[a] = 0.0;
             return;
         }
-        int dev = 0, sms = 148;
+        int dev = 0, sms = 132;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         const int blocks = (int)std::min<uint64_t>((uint64_t)sms * 8, (p.n + 255) / 256);

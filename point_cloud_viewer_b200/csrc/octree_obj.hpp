@@ -18,7 +18,7 @@ struct pcv_ctx {
     pcv_config cfg{};
     pcv::CudaBackend* be = nullptr;
     pcv_build_stats stats{};
-    int sm_count = 148;
+    int sm_count = 132;
     std::mutex mu;  // build / query entry points serialise on the context's stream
     // cells of the last pcv_prefix_histogram_device call, reused by the pack over the same points (shard_api.inl)
     uint16_t* shard_cells = nullptr;

@@ -1,5 +1,5 @@
 // pcv_api.cu — the C ABI (include/pcv.h) over the CUDA kernels.  One translation unit; built with
-//   nvcc -gencode arch=compute_100a,code=sm_100a -fmad=false -lineinfo ... (see __graft_entry__.build()).
+//   nvcc -gencode arch=compute_90a,code=sm_90a -fmad=false -lineinfo ... (see __graft_entry__.build()).
 // There is no CPU fallback in this library: every compute entry point needs a CUDA device.
 #include <cuda_runtime.h>
 #include <sys/stat.h>

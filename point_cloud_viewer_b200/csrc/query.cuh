@@ -1,4 +1,4 @@
-// query.cuh — sm_100a kernels of the query side.
+// query.cuh — sm_90a kernels of the query side.
 //
 //   k_sat_nodes      a11-a12  batched separating-axis test: (location, node cube) -> Relation
 //   k_propagate      a11      BFS semantics of NodeIdsIterator: a node is visited iff all ancestors passed

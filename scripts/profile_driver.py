@@ -1,5 +1,5 @@
 """One build of 1e8 benchmark points + one 200-frusta query batch + one 4096^2 X-ray tile: the kernels of the three measured
-workloads, once each, for `ncu --set full` (profiles/README.md)."""
+workloads, once each, for `ncu --set full`."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
