@@ -454,6 +454,35 @@ int pcv_ply_load_device(pcv_ctx* ctx, const char* path, const pcv_ply_info* info
  * mandatory; `with_intensity` mirrors "intensity" in the reference's `attributes` argument. */
 int pcv_build_octree_from_file(pcv_ctx* ctx, const char* path, double resolution, int with_intensity, pcv_octree** out);
 
+/* ---- out-of-core build_octree: clouds larger than one GPU's memory, straight into the on-disk octree ------------------
+ * The input streams through the GPU once to count the level-3 cells, then once per group: a group is a run of consecutive
+ * non-empty cells of the prefix level k actually used, filled up to the budget, and is built like one rank of
+ * pcv_build_octree_sharded; the nodes above level k come from pcv_assemble_top at the end.  The directory is byte for byte what
+ * pcv_build_octree[_from_file] + pcv_octree_write_dir write for the same input.  Device memory stays within one in-core build
+ * of the budget; the total point count may exceed 2^32 (each group and the nodes above level k stay below 2^32 - 1).
+ * A single level-k cell above the budget is PCV_ERR_UNSUPPORTED (the message names the cell, its count and the budget); that
+ * includes a cloud whose usable prefix level dropped because a node above it is a leaf. */
+/* Points one in-core build (pcv_build_octree[_device]) can take on this context now: free device memory over the build's
+ * per-point working set, capped at 2^32-2.  Also the default group budget below. */
+int pcv_in_core_capacity(pcv_ctx* ctx, int with_intensity, uint64_t* max_points);
+typedef struct pcv_ooc_info {
+    uint32_t prefix_levels; /* k actually used (1..3; 0 for an empty cloud)                              */
+    uint32_t groups;        /* in-core builds run                                                       */
+    uint64_t num_points, num_nodes, largest_group;
+    uint64_t h2d_bytes;     /* input bytes copied host -> device over all passes                         */
+    double ms_histogram, ms_select, ms_build, ms_write, ms_top, ms_total; /* wall clock, each phase ends in a stream sync;
+                                                                            ms_histogram includes a PLY file's bounding-box pass */
+} pcv_ooc_info;
+/* build_octree (generation.rs:289-295) for a cloud in host memory of any size (pageable or pinned, SoA or AoS like
+ * pcv_build_octree): writes <dir>/<NodeId>.xyz|.rgb|.intensity + meta.pb.  max_points_in_core = 0: pcv_in_core_capacity.
+ * info may be NULL. */
+int pcv_build_octree_to_dir(pcv_ctx* ctx, const pcv_points* host_points, double resolution, const double bbox_min[3],
+                            const double bbox_max[3], uint64_t max_points_in_core, const char* dir, pcv_ooc_info* info);
+/* build_octree_from_file (generation.rs:272-287) for a PLY file of any size: the body streams from disk on every pass (one
+ * bounding-box pass, one histogram pass, one pass per group). */
+int pcv_build_octree_from_file_to_dir(pcv_ctx* ctx, const char* ply_path, double resolution, int with_intensity,
+                                      uint64_t max_points_in_core, const char* dir, pcv_ooc_info* info);
+
 /* ---- synthetic inputs for benchmarks / parity tests (integer-only, counter based) ----------- */
 enum { PCV_SYNTH_SLAB_ECEF = 1, PCV_SYNTH_GAUSS_CLUSTERS = 2 };
 int pcv_synth_points_device(pcv_ctx* ctx, int kind, uint64_t seed, uint64_t first_index, uint64_t n, double* dev_x,

@@ -148,6 +148,33 @@ class Context:
         N.check(N.lib().pcv_build_octree_from_file(self.h, os.fsencode(str(path)), float(resolution), 1 if "intensity" in attributes else 0, C.byref(out)))
         return Octree(self, out)
 
+    # -- out-of-core build_octree: clouds larger than this GPU's memory, straight into the on-disk octree
+    def in_core_capacity(self, with_intensity=False):
+        """Points one in-core build_octree can take on this context now (free device memory over the build's working set)."""
+        out = C.c_uint64()
+        N.check(N.lib().pcv_in_core_capacity(self.h, 1 if with_intensity else 0, C.byref(out)))
+        return int(out.value)
+
+    def build_octree_to_dir(self, directory, x, y, z, rgb, resolution, bbox_min, bbox_max, intensity=None, stride=1, n=None, max_points_in_core=0):
+        """build_octree for host points of any size, written straight to `directory` (the same files as build_octree + write_dir)
+        in groups of at most `max_points_in_core` points (0: in_core_capacity).  Returns the pcv_ooc_info fields as a dict."""
+        if n is None:
+            n = len(rgb) // 3 if getattr(rgb, "ndim", 1) == 1 else rgb.shape[0]
+        keep = (x, y, z, rgb, intensity)
+        pts = N.Points(_p(x), _p(y), _p(z), stride, _p(rgb), _p(intensity), int(n))
+        info = N.OocInfo()
+        N.check(N.lib().pcv_build_octree_to_dir(self.h, C.byref(pts), float(resolution), _d3(bbox_min), _d3(bbox_max), int(max_points_in_core),
+                                                os.fsencode(str(directory)), C.byref(info)))
+        del keep
+        return {f: getattr(info, f) for f, _ in N.OocInfo._fields_}
+
+    def build_octree_from_file_to_dir(self, directory, path, resolution, attributes=("color",), max_points_in_core=0):
+        """build_octree_from_file for a PLY file of any size, written straight to `directory`.  Returns the pcv_ooc_info fields."""
+        info = N.OocInfo()
+        N.check(N.lib().pcv_build_octree_from_file_to_dir(self.h, os.fsencode(str(path)), float(resolution), 1 if "intensity" in attributes else 0,
+                                                          int(max_points_in_core), os.fsencode(str(directory)), C.byref(info)))
+        return {f: getattr(info, f) for f, _ in N.OocInfo._fields_}
+
     def load_dir(self, directory):
         out = C.c_void_p()
         N.check(N.lib().pcv_octree_load_dir(self.h, str(directory).encode(), C.byref(out)))
@@ -796,9 +823,17 @@ class PlyPoints:
 
 
 def build_octree_from_file(output_directory, resolution, filename, attributes=("color",), device=0, ctx=None):
-    """Drop-in shape of point_viewer::octree::build_octree_from_file (src/octree/generation.rs:272-287)."""
+    """Drop-in shape of point_viewer::octree::build_octree_from_file (src/octree/generation.rs:272-287).
+
+    With `ctx` the octree stays resident and is returned, unless the file holds more points than `ctx.in_core_capacity`: such a
+    file is built out of core straight into `output_directory` (Context.build_octree_from_file_to_dir) and None is returned."""
     own = ctx is None
     ctx = ctx or Context(device)
+    if int(ply_read_header(filename).num_points) > ctx.in_core_capacity("intensity" in attributes):
+        ctx.build_octree_from_file_to_dir(output_directory, filename, resolution, attributes)
+        if own:
+            ctx.close()
+        return None
     tree = ctx.build_octree_from_file(filename, resolution, attributes)
     tree.write_dir(output_directory)
     if own:
@@ -811,7 +846,10 @@ def build_octree_from_file(output_directory, resolution, filename, attributes=("
 def build_octree(output_directory, resolution, bounding_box, batches, attributes=("color",), device=0, ctx=None):
     """Drop-in shape of point_viewer::octree::build_octree (src/octree/generation.rs:289-295):
     drains `batches` (iterable of dict(position (n,3) f64, color (n,3) u8[, intensity (n,) f32])), builds on
-    the GPU, writes the reference's directory layout.  bounding_box = (min3, max3)."""
+    the GPU, writes the reference's directory layout.  bounding_box = (min3, max3).
+
+    With `ctx` the octree stays resident and is returned, unless the cloud holds more points than `ctx.in_core_capacity`: such a
+    cloud is built out of core straight into `output_directory` (Context.build_octree_to_dir) and None is returned."""
     pos, col, inten = [], [], []
     for b in batches:
         pos.append(np.ascontiguousarray(b["position"], np.float64).reshape(-1, 3))
@@ -824,6 +862,12 @@ def build_octree(output_directory, resolution, bounding_box, batches, attributes
     own = ctx is None
     ctx = ctx or Context(device)
     flat = P.reshape(-1)
+    if len(P) > ctx.in_core_capacity(I is not None):
+        ctx.build_octree_to_dir(output_directory, flat[0:], flat[1:], flat[2:], Cc.reshape(-1), resolution, bounding_box[0], bounding_box[1], intensity=I,
+                                stride=3, n=len(P))
+        if own:
+            ctx.close()
+        return None
     tree = ctx.build_octree(flat[0:], flat[1:], flat[2:], Cc.reshape(-1), resolution, bounding_box[0], bounding_box[1], intensity=I, stride=3, n=len(P))
     tree.write_dir(output_directory)
     if own:

@@ -149,6 +149,14 @@ class PlyInfo(C.Structure):
                 ("off_intensity", C.c_uint32), ("offset", C.c_double * 3)]
 
 
+class OocInfo(C.Structure):
+    """pcv_ooc_info (include/pcv.h)."""
+
+    _fields_ = [("prefix_levels", C.c_uint32), ("groups", C.c_uint32), ("num_points", C.c_uint64), ("num_nodes", C.c_uint64), ("largest_group", C.c_uint64),
+                ("h2d_bytes", C.c_uint64), ("ms_histogram", C.c_double), ("ms_select", C.c_double), ("ms_build", C.c_double), ("ms_write", C.c_double),
+                ("ms_top", C.c_double), ("ms_total", C.c_double)]
+
+
 # every symbol include/pcv.h declares: (name, restype, argtypes)
 _dp = C.POINTER(C.c_double)
 _u64p = C.POINTER(C.c_uint64)
@@ -231,6 +239,9 @@ SYMBOLS = [
     ("pcv_ply_unpack_device", C.c_int, [C.c_void_p, C.POINTER(PlyInfo), C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _dp, _dp]),
     ("pcv_ply_load_device", C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(PlyInfo), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _dp, _dp]),
     ("pcv_build_octree_from_file", C.c_int, [C.c_void_p, C.c_char_p, C.c_double, C.c_int, C.POINTER(C.c_void_p)]),
+    ("pcv_in_core_capacity", C.c_int, [C.c_void_p, C.c_int, _u64p]),
+    ("pcv_build_octree_to_dir", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_double, _dp, _dp, C.c_uint64, C.c_char_p, C.POINTER(OocInfo)]),
+    ("pcv_build_octree_from_file_to_dir", C.c_int, [C.c_void_p, C.c_char_p, C.c_double, C.c_int, C.c_uint64, C.c_char_p, C.POINTER(OocInfo)]),
     ("pcv_synth_points_device", C.c_int, [C.c_void_p, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("pcv_synth_points_host", C.c_int, [C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("pcv_synth_bbox", C.c_int, [C.c_int, _dp, _dp, _dp]),

@@ -90,7 +90,7 @@ constexpr int kMaxRanks = 64;
 
 struct PackArgs {
     PrefixArgs p;
-    const int32_t* cell_to_rank;  // device, nbins
+    const int32_t* cell_to_rank;  // device, nbins; a negative entry drops the cell's points (dest 0xFF, not counted, not stored)
     uint32_t nranks, ntiles;
     const uint16_t* cells;  // optional: level-(k + cell_shift / 3) cells from the histogram call over the same points
     uint32_t cell_shift;
@@ -101,7 +101,8 @@ struct PackArgs {
     double* out_xyz;          // n * 3 (AoS)
     uint8_t* out_rgb;
     float* out_intensity;
-    uint64_t* out_idx;
+    uint64_t* out_idx;        // optional
+    uint64_t out_base;        // first output slot of this call: successive calls over the chunks of one stream append
 };
 
 __global__ void __launch_bounds__(256) k_pack_count(const __grid_constant__ PackArgs a) {
@@ -113,8 +114,8 @@ __global__ void __launch_bounds__(256) k_pack_count(const __grid_constant__ Pack
     for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
         const unsigned cell = a.cells ? (unsigned)a.cells[t0 + i] >> a.cell_shift : prefix_cell(a.p, t0 + i);
         const int r = a.cell_to_rank[cell];
-        a.dest[t0 + i] = (uint8_t)r;
-        atomicAdd(&cnt[r], 1u);
+        a.dest[t0 + i] = r < 0 ? (uint8_t)0xFFu : (uint8_t)r;
+        if (r >= 0) atomicAdd(&cnt[r], 1u);
     }
     __syncthreads();
     if (threadIdx.x < a.nranks) a.counts[(size_t)threadIdx.x * a.ntiles + blockIdx.x] = cnt[threadIdx.x];
@@ -139,7 +140,7 @@ __global__ void __launch_bounds__(256) k_pack_scatter(const __grid_constant__ Pa
         uint32_t before = 0;
         if (d != 0xFFu) {
             for (int w = 0; w < warp; ++w) before += wc[w][d];
-            const uint64_t dst = (uint64_t)base[d] + before + rank;
+            const uint64_t dst = a.out_base + base[d] + before + rank;
             const uint64_t g = t0 + i;
             a.out_xyz[3 * dst] = __ldg(a.p.pts.x + g * a.p.pts.stride);
             a.out_xyz[3 * dst + 1] = __ldg(a.p.pts.y + g * a.p.pts.stride);
@@ -148,7 +149,7 @@ __global__ void __launch_bounds__(256) k_pack_scatter(const __grid_constant__ Pa
             a.out_rgb[3 * dst + 1] = __ldg(a.p.pts.rgb + 3 * g + 1);
             a.out_rgb[3 * dst + 2] = __ldg(a.p.pts.rgb + 3 * g + 2);
             if (a.out_intensity) a.out_intensity[dst] = __ldg(a.p.pts.intensity + g);
-            a.out_idx[dst] = a.gidx_in ? __ldg(a.gidx_in + g) : a.gidx_base + g;
+            if (a.out_idx) a.out_idx[dst] = a.gidx_in ? __ldg(a.gidx_in + g) : a.gidx_base + g;
         }
         __syncthreads();
         if (threadIdx.x < a.nranks) {

@@ -5,10 +5,12 @@
 #include <sys/stat.h>
 
 #include <cstdarg>
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
 #include <cstdio>
+#include <functional>
 #include <string>
 #include <memory>
 #include <thread>
@@ -16,6 +18,7 @@
 #include "../../include/pcv.h"
 #include "disk_io.hpp"
 #include "octree_obj.hpp"
+#include "ooc_plan.h"
 #include "ply.cuh"
 #include "ply_host.hpp"
 #include "kernels_shard.cuh"
@@ -484,41 +487,66 @@ int pcv_octree_device_arrays(const pcv_octree* o, const void** xyz, const uint8_
     return PCV_OK;
 }
 
+}  // extern "C"
+
+// Host copies of an octree's node-contiguous arrays (the caller holds the context's lock).
+struct HostArrays {
+    std::vector<uint8_t> xyz, rgb;
+    std::vector<float> inten;
+};
+static void download_arrays(const pcv_octree* o, HostArrays& h) {
+    pcv_ctx* c = o->ctx;
+    h.xyz.resize(o->xyz_bytes);
+    h.rgb.resize(o->n * 3);
+    h.inten.resize(o->has_intensity ? o->n : 0);
+    CU(cudaSetDevice(c->device));
+    if (!o->n) return;
+    CU(cudaMemcpyAsync(h.xyz.data(), o->d_xyz, o->xyz_bytes, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaMemcpyAsync(h.rgb.data(), o->d_rgb, o->n * 3, cudaMemcpyDeviceToHost, c->stream));
+    if (o->has_intensity) CU(cudaMemcpyAsync(h.inten.data(), o->d_intensity, o->n * 4, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+}
+
+// <dir>/<NodeId>.xyz|.rgb|.intensity of the nodes of `o` whose level is in [level_lo, level_hi), from the host copies.
+static void write_node_files(const std::string& d, const pcv_octree* o, const HostArrays& h, int level_lo, int level_hi) {
+    for (const auto& m : o->nodes) {
+        if (m.num_points == 0 || m.level < level_lo || m.level >= level_hi) continue;  // node_writer.rs:78-89: empty files do not exist
+        const std::string stem = d + "/" + node_name(m.id_high, m.id_low);
+        const uint64_t n = (uint64_t)m.num_points, bpc = (uint64_t)enc_bytes(m.position_encoding);
+        if (!write_whole_file(stem + ".xyz", h.xyz.data() + m.xyz_byte_offset, n * 3 * bpc) ||
+            !write_whole_file(stem + ".rgb", h.rgb.data() + 3 * m.point_offset, n * 3) ||
+            (o->has_intensity && !write_whole_file(stem + ".intensity", h.inten.data() + m.point_offset, n * 4)))
+            throw BuildError(PCV_ERR_IO, "cannot write node files " + stem + ".*");
+    }
+}
+
+// <dir>/meta.pb over `nodes` (sorted by NodeId)
+static void write_meta(const std::string& d, double resolution, const double bmin[3], const double bmax[3], const std::vector<pcv_node_meta>& nodes) {
+    MetaHeader h;
+    h.resolution = resolution;
+    for (int a = 0; a < 3; ++a) {
+        h.bbox_min[a] = bmin[a];
+        h.bbox_max[a] = bmax[a];
+    }
+    const std::string meta = encode_meta(h, nodes);
+    if (!write_whole_file(d + "/meta.pb", meta.data(), meta.size())) throw BuildError(PCV_ERR_IO, "cannot write " + d + "/meta.pb");
+}
+
+extern "C" {
+
 int pcv_octree_write_dir(const pcv_octree* o, const char* dir) {
     if (!o || !dir) return fail(PCV_ERR_INVALID, "null argument");
     API_TRY
     pcv_ctx* c = o->ctx;
     mkdir(dir, 0777);  // "Ignore errors, maybe directory is already there." generation.rs:306-307
-    std::vector<uint8_t> xyz(o->xyz_bytes), rgb(o->n * 3);
-    std::vector<float> inten(o->has_intensity ? o->n : 0);
+    HostArrays h;
     {
         std::lock_guard<std::mutex> g(c->mu);
-        CU(cudaSetDevice(c->device));
-        if (o->n) {
-            CU(cudaMemcpyAsync(xyz.data(), o->d_xyz, o->xyz_bytes, cudaMemcpyDeviceToHost, c->stream));
-            CU(cudaMemcpyAsync(rgb.data(), o->d_rgb, o->n * 3, cudaMemcpyDeviceToHost, c->stream));
-            if (o->has_intensity) CU(cudaMemcpyAsync(inten.data(), o->d_intensity, o->n * 4, cudaMemcpyDeviceToHost, c->stream));
-            CU(cudaStreamSynchronize(c->stream));
-        }
+        download_arrays(o, h);
     }
     const std::string d(dir);
-    for (const auto& m : o->nodes) {
-        if (m.num_points == 0) continue;  // node_writer.rs:78-89: empty files do not exist
-        const std::string stem = d + "/" + node_name(m.id_high, m.id_low);
-        const uint64_t n = (uint64_t)m.num_points, bpc = (uint64_t)enc_bytes(m.position_encoding);
-        if (!write_whole_file(stem + ".xyz", xyz.data() + m.xyz_byte_offset, n * 3 * bpc) ||
-            !write_whole_file(stem + ".rgb", rgb.data() + 3 * m.point_offset, n * 3) ||
-            (o->has_intensity && !write_whole_file(stem + ".intensity", inten.data() + m.point_offset, n * 4)))
-            return fail(PCV_ERR_IO, "cannot write node files %s.*", stem.c_str());
-    }
-    MetaHeader h;
-    h.resolution = o->resolution;
-    for (int a = 0; a < 3; ++a) {
-        h.bbox_min[a] = o->bbox_min[a];
-        h.bbox_max[a] = o->bbox_max[a];
-    }
-    const std::string meta = encode_meta(h, o->nodes);
-    if (!write_whole_file(d + "/meta.pb", meta.data(), meta.size())) return fail(PCV_ERR_IO, "cannot write %s/meta.pb", dir);
+    write_node_files(d, o, h, 0, INT32_MAX);
+    write_meta(d, o->resolution, o->bbox_min, o->bbox_max, o->nodes);
     return PCV_OK;
     API_CATCH
 }
@@ -668,3 +696,4 @@ int pcv_synth_bbox(int kind, double bbox_min[3], double bbox_max[3], double* res
 #include "ply_api.inl"
 #include "shard_api.inl"
 #include "sharded_build.inl"
+#include "ooc_build.inl"
