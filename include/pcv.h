@@ -213,10 +213,12 @@ int pcv_xray_assign_background(pcv_ctx* ctx, uint8_t* rgba, uint64_t num_pixels,
 int pcv_xray_build_parent(pcv_ctx* ctx, const uint8_t* const children[4], uint32_t child_px, const uint8_t background[4],
                           uint32_t tile_px, uint8_t* rgba_out /* tile_px * tile_px * 4 */);
 /* build_xray_quadtree (:560-622) as one call: bounding rect and levels (:515-533), every leaf tile at the deepest level
- * (:535-551, :624-667) with the chosen strategy, assign_background on the created leaves, then level by level the parents
- * (:669-693).  Every image stays in HBM until its parent is built; each finished tile is handed to `on_tile` (host
- * pointer, valid during the call; return non-zero to cancel -> PCV_ERR_CANCELLED; must not call into the same context).
- * What the reference writes as <id>.png and meta.pb is what on_tile receives plus `info`; PNG encoding stays on the host. */
+ * (:535-551, :624-667) with the chosen strategy, assign_background on the created leaves, and the parents (:669-693).  A leaf
+ * exists iff at least one point passes its location test (:489-504).  Each finished tile is handed to `on_tile` (host
+ * pointer, valid during the call; return non-zero to cancel -> PCV_ERR_CANCELLED; must not call into the same context) in
+ * post-order: every tile after all of its children, siblings in index order, the root last.  What the reference writes as
+ * <id>.png and meta.pb is what on_tile receives plus `info`; PNG encoding stays on the host.  pcv_xray_quadtree is
+ * pcv_xray_quadtree_bounded with max_device_bytes = 0. */
 typedef struct pcv_xray_quadtree_params {
     int32_t strategy;             /* 0 = XRay, or PCV_XRAY_COLORED / _INTENSITY / _HEIGHT_STDDEV                 */
     float p0, p1;                 /* as in pcv_xray_tile_attr                                                     */
@@ -248,6 +250,30 @@ int pcv_xray_quadtree(const pcv_octree* o, const pcv_xray_quadtree_params* param
  * tile_size, nodes; "meta.pb" for the root, "meta<digits>.pb" for a sub-root: xray/src/utils.rs:7-11, lib.rs:88-139). */
 int pcv_xray_quadtree_write_dir(const pcv_octree* o, const pcv_xray_quadtree_params* params, const char* directory,
                                 pcv_xray_quadtree_info* info_out);
+
+/* The same quadtree of any size in bounded device memory.  Leaves are made in blocks: the subtree of one quadtree node `block
+ * level` levels down from the root, all its leaves located with one batched node selection and binned by one kernel per key
+ * batch.  Above the block level at most four finished children per level wait for their parent.  Only quadtree nodes that a
+ * point of the octree falls into (with a margin) are enumerated, level by level from the root.  max_device_bytes bounds what
+ * the driver allocates besides the resident octree (0: most of the free device memory); a budget that cannot hold one leaf,
+ * or a leaf whose possible keys or working memory do not fit what the budget leaves, returns PCV_ERR_UNSUPPORTED.  A block
+ * holds at most 1 GiB of images, staged in as much page-locked host memory for delivery; the context's allocator cache is
+ * emptied after every block.  bounded_info_out may be NULL. */
+typedef struct pcv_xray_bounded_info {
+    uint64_t max_device_bytes;    /* the budget used                                                              */
+    uint64_t peak_device_bytes;   /* the most the driver held at once (the resident octree not counted)           */
+    uint64_t blocks_processed;    /* blocks at the block level whose subtree was visited                          */
+    uint64_t blocks_pruned;       /* block positions below the root never visited                                 */
+    uint64_t positions_evaluated; /* leaf positions tested with their exact location                              */
+    uint64_t key_batches;         /* XRay strategy: binning passes over a batch of leaves                         */
+    uint32_t block_level;         /* quadtree level of the block roots                                            */
+} pcv_xray_bounded_info;
+int pcv_xray_quadtree_bounded(const pcv_octree* o, const pcv_xray_quadtree_params* params, uint64_t max_device_bytes, pcv_xray_tile_fn on_tile,
+                              void* user, pcv_xray_quadtree_info* info_out, pcv_xray_bounded_info* bounded_info_out);
+/* ... written as pcv_xray_quadtree_write_dir writes it; the PNGs are encoded and written by a small pool of host threads
+ * behind a bounded queue while the device builds the next block. */
+int pcv_xray_quadtree_bounded_write_dir(const pcv_octree* o, const pcv_xray_quadtree_params* params, uint64_t max_device_bytes, const char* directory,
+                                        pcv_xray_quadtree_info* info_out, pcv_xray_bounded_info* bounded_info_out);
 
 /* ---- f4: the S2-cell point cloud (src/read_write/s2.rs, src/s2_cells/mod.rs, src/geometry/s2_cell_union.rs) ---- */
 /* Cell ids are the S2 library's 64-bit CellID values (face, Hilbert position, level marker bit); the arithmetic is the `s2`

@@ -203,10 +203,12 @@ class Octree {
         check(pcv_xray_tile_attr_binned(o_, tile.min.data(), tile.max.data(), w, h, query_from_global7, strategy, p0, p1, bin_size, rgba.data(), &any));
         return any != 0;
     }
-    // build_xray_quadtree (xray/src/generation.rs:560-622): every tile of the quadtree, leaves to root, through `on_tile`
-    // (level, index, RGBA tile_size_px^2); returns what the reference writes into the quadtree's meta.pb.
+    // build_xray_quadtree (xray/src/generation.rs:560-622): every tile of the quadtree through `on_tile` (level, index, RGBA
+    // tile_size_px^2) in post-order - every tile after all of its children, the root last; returns what the reference writes
+    // into the quadtree's meta.pb.  `max_device_bytes` bounds the driver's device memory (0: most of the free memory).
     template <class F>
-    pcv_xray_quadtree_info build_xray_quadtree(const pcv_xray_quadtree_params& params, F&& on_tile) const {
+    pcv_xray_quadtree_info build_xray_quadtree(const pcv_xray_quadtree_params& params, F&& on_tile, uint64_t max_device_bytes = 0,
+                                               pcv_xray_bounded_info* bounded_info = nullptr) const {
         struct Thunk {
             F* f;
             static int call(void* user, uint8_t level, uint64_t index, const uint8_t* rgba, uint32_t tile_px) {
@@ -215,7 +217,7 @@ class Octree {
             }
         } th{&on_tile};
         pcv_xray_quadtree_info info{};
-        check(pcv_xray_quadtree(o_, &params, &Thunk::call, &th, &info));
+        check(pcv_xray_quadtree_bounded(o_, &params, max_device_bytes, &Thunk::call, &th, &info, bounded_info));
         return info;
     }
     void write_to_directory(const std::string& dir) const { check(pcv_octree_write_dir(o_, dir.c_str())); }

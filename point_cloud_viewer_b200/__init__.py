@@ -627,17 +627,12 @@ class Octree:
         return bool(anyp.value), rgba
 
     def xray_quadtree(self, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0, query_from_global=None,
-                      background=(255, 255, 255, 255), root=(0, 0), on_tile=None, keep_tiles=True):
+                      background=(255, 255, 255, 255), root=(0, 0), on_tile=None, keep_tiles=True, max_device_bytes=0):
         """build_xray_quadtree (xray/src/generation.rs:560-622) on the GPU: returns (info dict, {(level, index): RGBA array}).
-        `on_tile(level, index, rgba)` is called for every finished tile (return a true value to cancel)."""
-        pr = N.XrayQuadtreeParams()
-        pr.strategy, pr.p0, pr.p1, pr.colormap, pr.bin_size = int(strategy), float(p0), float(p1), int(colormap), float(bin_size)
-        pr.has_query_from_global = 0 if query_from_global is None else 1
-        if query_from_global is not None:
-            pr.query_from_global = (C.c_double * 7)(*[float(v) for v in query_from_global])
-        pr.background = (C.c_uint8 * 4)(*[int(v) for v in background])
-        pr.tile_size_px, pr.pixel_size_m = int(tile_size_px), float(pixel_size_m)
-        pr.root_level, pr.root_index = int(root[0]), int(root[1])
+        `on_tile(level, index, rgba)` is called for every finished tile in post-order, every tile after its children (return a
+        true value to cancel).  `max_device_bytes` bounds the driver's device memory (0: most of the free memory); the info
+        dict holds the pcv_xray_quadtree_info and pcv_xray_bounded_info fields."""
+        pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
         tiles = {}
 
         def cb(_user, level, index, ptr, tpx):
@@ -646,17 +641,18 @@ class Octree:
                 tiles[(int(level), int(index))] = img.copy()
             return 1 if (on_tile is not None and on_tile(int(level), int(index), img)) else 0
 
-        info = N.XrayQuadtreeInfo()
-        N.check(N.lib().pcv_xray_quadtree(self.h, C.byref(pr), N.XRAY_TILE_FN(cb), None, C.byref(info)))
-        return {k: getattr(info, k) for k, _ in N.XrayQuadtreeInfo._fields_}, tiles
+        info, binfo = N.XrayQuadtreeInfo(), N.XrayBoundedInfo()
+        N.check(N.lib().pcv_xray_quadtree_bounded(self.h, C.byref(pr), int(max_device_bytes), N.XRAY_TILE_FN(cb), None, C.byref(info), C.byref(binfo)))
+        return _xray_info(info, binfo), tiles
 
     def xray_quadtree_write_dir(self, directory, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0, query_from_global=None,
-                                background=(255, 255, 255, 255), root=(0, 0)):
+                                background=(255, 255, 255, 255), root=(0, 0), max_device_bytes=0):
         """build_xray_quadtree with the reference's outputs: <directory>/<node id>.png + the quadtree's meta file."""
         pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
-        info = N.XrayQuadtreeInfo()
-        N.check(N.lib().pcv_xray_quadtree_write_dir(self.h, C.byref(pr), os.fsencode(str(directory)), C.byref(info)))
-        return {k: getattr(info, k) for k, _ in N.XrayQuadtreeInfo._fields_}
+        info, binfo = N.XrayQuadtreeInfo(), N.XrayBoundedInfo()
+        N.check(N.lib().pcv_xray_quadtree_bounded_write_dir(self.h, C.byref(pr), int(max_device_bytes), os.fsencode(str(directory)), C.byref(info),
+                                                            C.byref(binfo)))
+        return _xray_info(info, binfo)
 
 
 class S2Cloud:
@@ -753,6 +749,12 @@ def _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_siz
     pr.tile_size_px, pr.pixel_size_m = int(tile_size_px), float(pixel_size_m)
     pr.root_level, pr.root_index = int(root[0]), int(root[1])
     return pr
+
+
+def _xray_info(info, binfo):
+    out = {k: getattr(info, k) for k, _ in N.XrayQuadtreeInfo._fields_}
+    out.update({k: getattr(binfo, k) for k, _ in N.XrayBoundedInfo._fields_})
+    return out
 
 
 def xray_assign_background(ctx, rgba, background):

@@ -125,6 +125,13 @@ class XrayQuadtreeInfo(C.Structure):
                 ("ms_parents", C.c_float), ("kernel_launches", C.c_uint32), ("leaf_points", C.c_uint64)]
 
 
+class XrayBoundedInfo(C.Structure):
+    """pcv_xray_bounded_info (include/pcv.h)."""
+
+    _fields_ = [("max_device_bytes", C.c_uint64), ("peak_device_bytes", C.c_uint64), ("blocks_processed", C.c_uint64), ("blocks_pruned", C.c_uint64),
+                ("positions_evaluated", C.c_uint64), ("key_batches", C.c_uint64), ("block_level", C.c_uint32)]
+
+
 XRAY_TILE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint8, C.c_uint64, C.POINTER(C.c_uint8), C.c_uint32)
 
 
@@ -193,6 +200,10 @@ SYMBOLS = [
     ("pcv_xray_build_parent", C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p]),
     ("pcv_xray_quadtree", C.c_int, [C.c_void_p, C.POINTER(XrayQuadtreeParams), XRAY_TILE_FN, C.c_void_p, C.POINTER(XrayQuadtreeInfo)]),
     ("pcv_xray_quadtree_write_dir", C.c_int, [C.c_void_p, C.POINTER(XrayQuadtreeParams), C.c_char_p, C.POINTER(XrayQuadtreeInfo)]),
+    ("pcv_xray_quadtree_bounded", C.c_int, [C.c_void_p, C.POINTER(XrayQuadtreeParams), C.c_uint64, XRAY_TILE_FN, C.c_void_p, C.POINTER(XrayQuadtreeInfo),
+                                            C.POINTER(XrayBoundedInfo)]),
+    ("pcv_xray_quadtree_bounded_write_dir", C.c_int, [C.c_void_p, C.POINTER(XrayQuadtreeParams), C.c_uint64, C.c_char_p, C.POINTER(XrayQuadtreeInfo),
+                                                      C.POINTER(XrayBoundedInfo)]),
     ("pcv_s2_cell_ids", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_uint32, C.c_void_p]),
     ("pcv_s2_build", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_uint32, C.POINTER(C.c_void_p)]),
     ("pcv_s2_build_device", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_uint32, C.POINTER(C.c_void_p)]),

@@ -732,21 +732,151 @@ __global__ void __launch_bounds__(256) k_xray_bin(const __grid_constant__ XrayBi
         }
     }
 }
+// The same binning for a batch of leaf tiles of one quadtree (the bounded quadtree driver, xray_api.inl): every work tile
+// carries its leaf in `loc`, every leaf has its own location and box (leaves[loc]; transform, w and h are shared), and the bins
+// are (leaf, sub-tile) pairs, leaf-major: bin = leaf * nsub + sub.  A point on an edge shared by two leaves goes into every
+// leaf whose closed box contains it (the work list holds one tile per (leaf, node) pair).  The count pass also raises
+// seen[leaf] for every point that passes the leaf's location test: the leaf exists iff one does (generation.rs:489-504).
+struct XrayBatchArgs {
+    const XrayArgs* leaves;   // [nleaf] geom, tmin, tdiag, rdiag, div_ok, query_from_global, has_q, w, h of every leaf
+    const QNode* nodes;
+    const QTile* tiles;
+    const uint8_t* xyz;
+    uint32_t ntiles;
+    uint32_t sub_w, nsub;     // sub-tiles per row and per leaf
+    uint32_t* sub_count;      // [nleaf * nsub + 1]; after the scan: exclusive offsets
+    uint32_t* sub_cursor;     // [nleaf * nsub]
+    uint32_t* keys;
+    int* seen;                // [nleaf]
+};
+template <int PLACE>
+__global__ void __launch_bounds__(256) k_xray_bin_batch(const __grid_constant__ XrayBatchArgs b) {
+    const int lane = threadIdx.x & 31;
+    for (uint32_t ti = blockIdx.x; ti < b.ntiles; ti += gridDim.x) {
+        const QTile t = b.tiles[ti];
+        const XrayArgs& a = b.leaves[t.loc];
+        const QNode nd = b.nodes[t.node];
+        const int bpc = enc_bytes(nd.enc);
+        bool seen = false;
+        for (uint32_t i0 = 0; i0 < t.count; i0 += blockDim.x) {
+            const uint32_t i = i0 + threadIdx.x;
+            uint32_t bin = 0xFFFFFFFFu, key = 0;
+            if (i < t.count) {
+                const uint8_t* s = b.xyz + nd.xyz_off + (uint64_t)(t.first + i) * 3 * bpc;
+                double p[3];
+#pragma unroll
+                for (int k = 0; k < 3; ++k) p[k] = decode1_fast(load_code(s + k * bpc, nd.enc), nd.m[k], nd.e, nd.enc);
+                if (loc_contains(a.geom, p[0], p[1], p[2])) {
+                    seen = true;
+                    if (a.has_q) {  // generation.rs:493-497
+                        const V3 q = iso_apply(a.query_from_global, V3{p[0], p[1], p[2]});
+                        p[0] = q.x, p[1] = q.y, p[2] = q.z;
+                    }
+                    // process_point_data, generation.rs:108-127, exactly as in k_xray_bin
+                    const uint32_t x = rust_as_u32_dev(xray_unit(a, 0, p[0]) * (double)a.w);
+                    const uint32_t y = rust_as_u32_dev((1. - xray_unit(a, 1, p[1])) * (double)a.h);
+                    const uint32_t z = rust_as_u32_dev(xray_unit(a, 2, p[2]) * 1024.);
+                    if (x < a.w && y < a.h) {
+                        bin = t.loc * b.nsub + (y / kXraySub) * b.sub_w + (x / kXraySub);
+                        key = ((y % kXraySub) << 16) | ((x % kXraySub) << 11) | min(z, 1024u);
+                    }
+                }
+            }
+            // one atomic per warp and distinct bin
+            const unsigned mask = __match_any_sync(0xffffffffu, bin);
+            if (bin != 0xFFFFFFFFu) {
+                const int leader = __ffs(mask) - 1;
+                const uint32_t rank = __popc(mask & ((1u << lane) - 1u));
+                if (PLACE) {
+                    uint32_t base = 0;
+                    if (lane == leader) base = atomicAdd(&b.sub_cursor[bin], (uint32_t)__popc(mask));
+                    base = __shfl_sync(mask, base, leader);
+                    b.keys[b.sub_count[bin] + base + rank] = key;
+                } else if (lane == leader) {
+                    atomicAdd(&b.sub_count[bin], (uint32_t)__popc(mask));
+                }
+            }
+        }
+        if (!PLACE && __syncthreads_or(seen) && threadIdx.x == 0) b.seen[t.loc] = 1;
+    }
+}
+// Which candidate quadtree nodes of one level can hold a point (the pruning of the bounded quadtree driver).  Every point of
+// the octree (interior nodes hold points too, so node cubes cannot tell an empty area from a full one) is decoded, moved
+// into the quadtree's frame like k_xray_bin does, and marks every candidate whose cell - the level's grid over the quadtree
+// rect, widened by `margin` on each side - contains it: at most four cells, found by binary search in the sorted candidates.
+struct XrayOccupyArgs {
+    const QNode* nodes;
+    const QTile* tiles;       // every node's points
+    const uint8_t* xyz;
+    uint32_t ntiles;
+    double query_from_global[7];
+    int has_q;
+    double x0, y0, edge;      // the quadtree rect's minimum, the edge of one node of the level
+    double margin;
+    uint32_t level;
+    const unsigned long long* cand;  // sorted node indices of the level
+    uint32_t ncand;
+    uint32_t* hit;            // [ncand]
+};
+__device__ __forceinline__ void xray_cell_range(double v, double v0, double edge, double margin, uint64_t cells, int64_t& lo, int64_t& hi) {
+    const double a = floor((v - margin - v0) / edge), b = floor((v + margin - v0) / edge);
+    lo = 1, hi = 0;  // empty
+    if (!(a == a) || !(b == b) || b < 0.0 || a >= (double)cells) return;
+    lo = a < 0.0 ? 0 : (int64_t)a;
+    hi = b >= (double)cells ? (int64_t)cells - 1 : (int64_t)b;
+}
+__global__ void __launch_bounds__(256) k_xray_occupy(const __grid_constant__ XrayOccupyArgs a) {
+    const uint64_t cells = 1ull << a.level;
+    for (uint32_t ti = blockIdx.x; ti < a.ntiles; ti += gridDim.x) {
+        const QTile t = a.tiles[ti];
+        const QNode nd = a.nodes[t.node];
+        const int bpc = enc_bytes(nd.enc);
+        for (uint32_t i = threadIdx.x; i < t.count; i += blockDim.x) {
+            const uint8_t* s = a.xyz + nd.xyz_off + (uint64_t)(t.first + i) * 3 * bpc;
+            double p[3];
+#pragma unroll
+            for (int k = 0; k < 3; ++k) p[k] = decode1_fast(load_code(s + k * bpc, nd.enc), nd.m[k], nd.e, nd.enc);
+            if (a.has_q) {
+                const V3 q = iso_apply(a.query_from_global, V3{p[0], p[1], p[2]});
+                p[0] = q.x, p[1] = q.y;
+            }
+            int64_t x0, x1, y0, y1;
+            xray_cell_range(p[0], a.x0, a.edge, a.margin, cells, x0, x1);
+            xray_cell_range(p[1], a.y0, a.edge, a.margin, cells, y0, y1);
+            for (int64_t ix = x0; ix <= x1; ++ix)
+                for (int64_t iy = y0; iy <= y1; ++iy) {
+                    uint64_t idx = 0;  // quadtree child k: bit 1 -> +x, bit 0 -> +y (quadtree lib.rs:84-101)
+                    for (uint32_t b = 0; b < a.level; ++b) idx |= ((((uint64_t)ix >> b) & 1ull) << (2 * b + 1)) | ((((uint64_t)iy >> b) & 1ull) << (2 * b));
+                    uint32_t l = 0, h = a.ncand;
+                    while (l < h) {
+                        const uint32_t m = (l + h) >> 1;
+                        if (a.cand[m] < idx)
+                            l = m + 1;
+                        else
+                            h = m;
+                    }
+                    if (l < a.ncand && a.cand[l] == idx && !a.hit[l]) a.hit[l] = 1;
+                }
+        }
+    }
+}
 struct XraySubArgs {
     const uint32_t* sub_id;     // unused (every sub-tile has a block; empty ones leave at once)
-    const uint32_t* sub_off;    // [nsub + 1] exclusive offsets into keys
+    const uint32_t* sub_off;    // [nleaf * nsub + 1] exclusive offsets into keys
     const uint32_t* keys;
     const uint8_t* grey;        // [1026]
-    uint8_t* rgba;              // w * h * 4, zero-initialised
-    uint32_t* zbits_out;        // optional: w * h * 32, zero-initialised
+    uint8_t* rgba;              // nleaf images of w * h * 4, one after the other, pre-filled with TRANSPARENT
+    uint32_t* zbits_out;        // optional (a single leaf): w * h * 32, zero-initialised
     uint32_t sub_w, w, h;
+    uint32_t nsub;              // sub-tiles per leaf image: block b resolves sub-tile b % nsub of image b / nsub
 };
 __global__ void __launch_bounds__(512, 1) k_xray_subtile(const __grid_constant__ XraySubArgs b) {
     extern __shared__ __align__(16) uint32_t sbits[];  // [1024 pixels][32 words]
     __shared__ uint8_t sover[kXraySub * kXraySub];
-    const uint32_t sid = blockIdx.x;
-    const uint32_t k0 = b.sub_off[sid], k1 = b.sub_off[sid + 1];
+    const uint32_t k0 = b.sub_off[blockIdx.x], k1 = b.sub_off[blockIdx.x + 1];
     if (k1 == k0) return;  // no point falls into this sub-tile: its pixels stay transparent (the image is pre-filled with TRANSPARENT)
+    const uint32_t sid = blockIdx.x % b.nsub;
+    uint8_t* const rgba = b.rgba + (size_t)(blockIdx.x / b.nsub) * b.w * b.h * 4;
     const uint32_t px0 = (sid % b.sub_w) * kXraySub, py0 = (sid / b.sub_w) * kXraySub;
     {
         uint4* z4 = reinterpret_cast<uint4*>(sbits);
@@ -777,7 +907,7 @@ __global__ void __launch_bounds__(512, 1) k_xray_subtile(const __grid_constant__
         for (int k = 0; k < 32; ++k) cnt += __popc(sbits[lp * 32 + ((k + lp) & 31)]);  // rotated start: no 32-way bank conflict
         if (cnt) {
             const uint8_t gv = b.grey[cnt];
-            reinterpret_cast<uchar4*>(b.rgba)[(size_t)y * b.w + x] = make_uchar4(gv, gv, gv, 255);
+            reinterpret_cast<uchar4*>(rgba)[(size_t)y * b.w + x] = make_uchar4(gv, gv, gv, 255);
         }
         if (b.zbits_out) {
             uint32_t* o = b.zbits_out + ((size_t)y * b.w + x) * 32;

@@ -1,0 +1,78 @@
+// xray_plan.h — host-only planning of the bounded X-ray quadtree driver (xray_api.inl; no CUDA: the CPU tests compile it with g++).
+//   xray_block_depth:     how many quadtree levels one block of leaves spans, from the device-memory budget
+//   xray_key_batches:     consecutive leaves of a block grouped so that their possible keys fit the key buffer
+//   xray_levels_to_close: the post-order bookkeeping - which ancestors are complete when the walk moves on to the next subtree
+//   xray_post_order:      every node of a subtree with the given leaves, each after all of its children
+#pragma once
+#include <cstdint>
+#include <utility>
+#include <vector>
+
+namespace pcv {
+
+// Device bytes of the images at block depth g (the block root is g levels above the leaves) under `above` levels between the
+// quadtree root and the block root:
+//   - the block's leaf images, 4^g of them at most, and its parents up to the block root, (4^g - 1) / 3 of them (every level
+//     of the block stays until the block root is built, so that the block leaves the device in one copy per level);
+//   - per level above the block at most four finished children wait for their parent, plus the parent being built.
+// `leaf_bytes` is everything the driver holds per leaf (image, bins, arguments); `tile_bytes` one RGBA tile.
+inline uint64_t xray_block_bytes(int g, int above, uint64_t leaf_bytes, uint64_t tile_bytes) {
+    const uint64_t leaves = 1ull << (2 * g), parents = (leaves - 1) / 3;
+    return leaves * leaf_bytes + parents * tile_bytes + (4ull * (uint64_t)above + 1) * tile_bytes;
+}
+
+// Largest g <= min(depth, max_g) whose images take at most half of what the budget leaves after `fixed_bytes` (the other half
+// holds the keys of a batch and the node selection); g = 0 when only a single leaf fits that way but fits the whole budget.
+// -1: not even one leaf fits the budget.
+inline int xray_block_depth(uint64_t budget, uint64_t fixed_bytes, int depth, int max_g, uint64_t leaf_bytes, uint64_t tile_bytes) {
+    if (budget <= fixed_bytes || xray_block_bytes(0, depth, leaf_bytes, tile_bytes) > budget - fixed_bytes) return -1;
+    const uint64_t half = (budget - fixed_bytes) / 2;
+    int g = 0;
+    while (g < depth && g < max_g && xray_block_bytes(g + 1, depth - g - 1, leaf_bytes, tile_bytes) <= half) ++g;
+    return g;
+}
+
+// Key batches over the leaves of a block, in order: each batch is a run of consecutive leaves whose possible keys (`keys[i]`,
+// one per point the leaf's location can hold) sum to at most `key_cap`.  Returns the batch starts plus an end sentinel, or an
+// empty vector with `*too_big` = the first leaf that alone exceeds key_cap.
+inline std::vector<uint32_t> xray_key_batches(const std::vector<uint64_t>& keys, uint64_t key_cap, int64_t* too_big) {
+    std::vector<uint32_t> starts;
+    *too_big = -1;
+    uint64_t run = 0;
+    for (size_t i = 0; i < keys.size(); ++i) {
+        if (keys[i] > key_cap) {
+            *too_big = (int64_t)i;
+            return {};
+        }
+        if (starts.empty() || run + keys[i] > key_cap) {
+            starts.push_back((uint32_t)i);
+            run = 0;
+        }
+        run += keys[i];
+    }
+    starts.push_back((uint32_t)keys.size());
+    return starts;
+}
+
+// a and b (a < b) are node indices `depth` levels below a common subtree root.  Returns how many ancestors of a are complete
+// when the post-order walk moves from a's subtree to b's: those at 1, 2, ..., k levels above a (never the common root).
+inline int xray_levels_to_close(uint64_t a, uint64_t b, int depth) {
+    int k = 0;
+    for (int up = 1; up < depth && (a >> (2 * up)) != (b >> (2 * up)); ++up) ++k;
+    return k;
+}
+
+// Post-order of the subtree that holds exactly the ancestors of the given leaves: `leaves` are sorted, distinct indices
+// `depth` levels below the subtree root.  Each entry is (levels above the leaves, index at that level); siblings come in
+// index order, every node after its children, the subtree root last.
+inline std::vector<std::pair<int, uint64_t>> xray_post_order(const std::vector<uint64_t>& leaves, int depth) {
+    std::vector<std::pair<int, uint64_t>> out;
+    for (size_t i = 0; i < leaves.size(); ++i) {
+        out.emplace_back(0, leaves[i]);
+        const int k = i + 1 < leaves.size() ? xray_levels_to_close(leaves[i], leaves[i + 1], depth) : depth;
+        for (int up = 1; up <= k; ++up) out.emplace_back(up, leaves[i] >> (2 * up));
+    }
+    return out;
+}
+
+}  // namespace pcv
