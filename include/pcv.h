@@ -275,6 +275,37 @@ int pcv_xray_quadtree_bounded(const pcv_octree* o, const pcv_xray_quadtree_param
 int pcv_xray_quadtree_bounded_write_dir(const pcv_octree* o, const pcv_xray_quadtree_params* params, uint64_t max_device_bytes, const char* directory,
                                         pcv_xray_quadtree_info* info_out, pcv_xray_bounded_info* bounded_info_out);
 
+/* The same quadtree straight from an octree directory (meta.pb + node files, as pcv_octree_write_dir and
+ * pcv_build_octree_to_dir leave it), which is never resident as a whole: the same tiles, post-order, cancellation and outputs as
+ * pcv_xray_quadtree_bounded over pcv_octree_load_dir of the directory.  One streaming pass over every node's positions marks
+ * the leaves a point falls into (with the driver's margin); then each block of leaves runs on its window, the nodes the block's
+ * location (widened by the margin) can meet, read from disk.  Nodes the previous window holds are copied on the device when the
+ * budget has room for both.  Here max_device_bytes bounds everything the call allocates, the windows included (0: most of the
+ * free device memory).  Host memory holds the largest window, the occupied leaves and the driver's staging.  Errors: a meta.pb
+ * other than version 13 -> PCV_ERR_INVALID; a missing or wrongly sized .xyz / .rgb file -> PCV_ERR_NOT_FOUND; a leaf whose window
+ * alone does not fit the budget or holds 2^32 points or more -> PCV_ERR_UNSUPPORTED.  bounded_info_out and dir_info_out may be NULL. */
+typedef struct pcv_xray_dir_info {
+    uint64_t windows_loaded;        /* blocks whose window was loaded                                               */
+    uint64_t node_files_read;       /* .xyz / .rgb / .intensity files read, the occupancy pass included             */
+    uint64_t bytes_read;            /* bytes read from those files                                                  */
+    uint64_t nodes_reread;          /* window nodes read again from disk after an earlier window had loaded them    */
+    uint64_t nodes_reused;          /* window nodes copied on the device from the previous window                   */
+    uint64_t bytes_reused;          /* bytes of those copies                                                        */
+    uint64_t bytes_uploaded;        /* host -> device bytes of node data (occupancy pass and windows)               */
+    uint64_t largest_window_bytes;  /* device bytes of the largest window (arrays and query tables)                 */
+    uint64_t largest_window_points;
+    uint64_t occupied_leaves;       /* leaves the occupancy pass marked                                             */
+    double ms_occupancy;            /* wall time of the occupancy pass                                              */
+    double ms_windows;              /* wall time of window planning and loading (reads, uploads, query tables)      */
+} pcv_xray_dir_info;
+int pcv_xray_quadtree_from_dir(pcv_ctx* ctx, const char* octree_dir, const pcv_xray_quadtree_params* params, uint64_t max_device_bytes,
+                               pcv_xray_tile_fn on_tile, void* user, pcv_xray_quadtree_info* info_out, pcv_xray_bounded_info* bounded_info_out,
+                               pcv_xray_dir_info* dir_info_out);
+/* ... written as pcv_xray_quadtree_bounded_write_dir writes it. */
+int pcv_xray_quadtree_from_dir_write_dir(pcv_ctx* ctx, const char* octree_dir, const pcv_xray_quadtree_params* params, uint64_t max_device_bytes,
+                                         const char* out_dir, pcv_xray_quadtree_info* info_out, pcv_xray_bounded_info* bounded_info_out,
+                                         pcv_xray_dir_info* dir_info_out);
+
 /* ---- f4: the S2-cell point cloud (src/read_write/s2.rs, src/s2_cells/mod.rs, src/geometry/s2_cell_union.rs) ---- */
 /* Cell ids are the S2 library's 64-bit CellID values (face, Hilbert position, level marker bit); the arithmetic is the `s2`
  * crate's, restated (csrc/s2.h): integer and IEEE +, *, /, sqrt only, identical on host and device. */

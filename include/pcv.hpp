@@ -121,6 +121,23 @@ class Context {
     Context(const Context&) = delete;
     Context& operator=(const Context&) = delete;
     pcv_ctx* raw() const { return h_; }
+    // build_xray_quadtree over the octree in `octree_dir` (build_quadtree.rs), streamed from disk window by window: what
+    // Octree::build_xray_quadtree gives over the loaded directory.  `max_device_bytes` bounds everything the call allocates.
+    template <class F>
+    pcv_xray_quadtree_info build_xray_quadtree_from_dir(const std::string& octree_dir, const pcv_xray_quadtree_params& params, F&& on_tile,
+                                                        uint64_t max_device_bytes = 0, pcv_xray_bounded_info* bounded_info = nullptr,
+                                                        pcv_xray_dir_info* dir_info = nullptr) const {
+        struct Thunk {
+            F* f;
+            static int call(void* user, uint8_t level, uint64_t index, const uint8_t* rgba, uint32_t tile_px) {
+                (*static_cast<Thunk*>(user)->f)(level, index, rgba, tile_px);
+                return 0;
+            }
+        } th{&on_tile};
+        pcv_xray_quadtree_info info{};
+        check(pcv_xray_quadtree_from_dir(h_, octree_dir.c_str(), &params, max_device_bytes, &Thunk::call, &th, &info, bounded_info, dir_info));
+        return info;
+    }
 
    private:
     pcv_ctx* h_ = nullptr;

@@ -175,6 +175,35 @@ class Context:
                                                           int(max_points_in_core), os.fsencode(str(directory)), C.byref(info)))
         return {f: getattr(info, f) for f, _ in N.OocInfo._fields_}
 
+    # -- X-ray quadtrees straight from an octree directory (never resident as a whole)
+    def xray_quadtree_from_dir(self, octree_dir, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0,
+                               query_from_global=None, background=(255, 255, 255, 255), root=(0, 0), on_tile=None, keep_tiles=True, max_device_bytes=0):
+        """Octree.xray_quadtree over the octree in `octree_dir`, streamed from disk window by window: the same (info dict, tiles)
+        and keywords.  `max_device_bytes` bounds everything the call allocates (0: most of the free memory); the info dict also
+        holds the pcv_xray_dir_info fields."""
+        pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
+        tiles = {}
+
+        def cb(_user, level, index, ptr, tpx):
+            img = np.ctypeslib.as_array(ptr, shape=(tpx, tpx, 4))
+            if keep_tiles:
+                tiles[(int(level), int(index))] = img.copy()
+            return 1 if (on_tile is not None and on_tile(int(level), int(index), img)) else 0
+
+        info, binfo, dinfo = N.XrayQuadtreeInfo(), N.XrayBoundedInfo(), N.XrayDirInfo()
+        N.check(N.lib().pcv_xray_quadtree_from_dir(self.h, os.fsencode(str(octree_dir)), C.byref(pr), int(max_device_bytes), N.XRAY_TILE_FN(cb), None,
+                                                   C.byref(info), C.byref(binfo), C.byref(dinfo)))
+        return _xray_info(info, binfo, dinfo), tiles
+
+    def xray_quadtree_from_dir_write_dir(self, octree_dir, out_dir, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0,
+                                         query_from_global=None, background=(255, 255, 255, 255), root=(0, 0), max_device_bytes=0):
+        """xray_quadtree_from_dir with the reference's outputs: <out_dir>/<node id>.png + the quadtree's meta file."""
+        pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
+        info, binfo, dinfo = N.XrayQuadtreeInfo(), N.XrayBoundedInfo(), N.XrayDirInfo()
+        N.check(N.lib().pcv_xray_quadtree_from_dir_write_dir(self.h, os.fsencode(str(octree_dir)), C.byref(pr), int(max_device_bytes),
+                                                             os.fsencode(str(out_dir)), C.byref(info), C.byref(binfo), C.byref(dinfo)))
+        return _xray_info(info, binfo, dinfo)
+
     def load_dir(self, directory):
         out = C.c_void_p()
         N.check(N.lib().pcv_octree_load_dir(self.h, str(directory).encode(), C.byref(out)))
@@ -751,9 +780,11 @@ def _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_siz
     return pr
 
 
-def _xray_info(info, binfo):
+def _xray_info(info, binfo, dinfo=None):
     out = {k: getattr(info, k) for k, _ in N.XrayQuadtreeInfo._fields_}
     out.update({k: getattr(binfo, k) for k, _ in N.XrayBoundedInfo._fields_})
+    if dinfo is not None:
+        out.update({k: getattr(dinfo, k) for k, _ in N.XrayDirInfo._fields_})
     return out
 
 

@@ -132,6 +132,14 @@ class XrayBoundedInfo(C.Structure):
                 ("positions_evaluated", C.c_uint64), ("key_batches", C.c_uint64), ("block_level", C.c_uint32)]
 
 
+class XrayDirInfo(C.Structure):
+    """pcv_xray_dir_info (include/pcv.h)."""
+
+    _fields_ = [("windows_loaded", C.c_uint64), ("node_files_read", C.c_uint64), ("bytes_read", C.c_uint64), ("nodes_reread", C.c_uint64),
+                ("nodes_reused", C.c_uint64), ("bytes_reused", C.c_uint64), ("bytes_uploaded", C.c_uint64), ("largest_window_bytes", C.c_uint64),
+                ("largest_window_points", C.c_uint64), ("occupied_leaves", C.c_uint64), ("ms_occupancy", C.c_double), ("ms_windows", C.c_double)]
+
+
 XRAY_TILE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint8, C.c_uint64, C.POINTER(C.c_uint8), C.c_uint32)
 
 
@@ -204,6 +212,10 @@ SYMBOLS = [
                                             C.POINTER(XrayBoundedInfo)]),
     ("pcv_xray_quadtree_bounded_write_dir", C.c_int, [C.c_void_p, C.POINTER(XrayQuadtreeParams), C.c_uint64, C.c_char_p, C.POINTER(XrayQuadtreeInfo),
                                                       C.POINTER(XrayBoundedInfo)]),
+    ("pcv_xray_quadtree_from_dir", C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(XrayQuadtreeParams), C.c_uint64, XRAY_TILE_FN, C.c_void_p,
+                                             C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo), C.POINTER(XrayDirInfo)]),
+    ("pcv_xray_quadtree_from_dir_write_dir", C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(XrayQuadtreeParams), C.c_uint64, C.c_char_p,
+                                                       C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo), C.POINTER(XrayDirInfo)]),
     ("pcv_s2_cell_ids", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_uint32, C.c_void_p]),
     ("pcv_s2_build", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_uint32, C.POINTER(C.c_void_p)]),
     ("pcv_s2_build_device", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_uint32, C.POINTER(C.c_void_p)]),

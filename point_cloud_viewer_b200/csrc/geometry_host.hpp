@@ -184,6 +184,57 @@ inline QueryGeom make_query_geom(const pcv_location& loc) {
     return g;
 }
 
+// The location of an X-ray tile with box [tmin, tmax]: Aabb(bbox), or Obb::from(bbox).transformed(query_from_global.inverse())
+// (xray generation.rs:471-477).
+inline pcv_location xray_location(const double tmin[3], const double tmax[3], const double* qfg) {
+    pcv_location loc{};
+    double bmin[3], bmax[3];
+    for (int a = 0; a < 3; ++a) {
+        bmin[a] = std::fmin(tmin[a], tmax[a]);
+        bmax[a] = std::fmax(tmin[a], tmax[a]);
+    }
+    if (qfg) {
+        loc.kind = PCV_LOC_OBB;
+        double ginv[7];  // global_from_query = query_from_global.inverse(): conjugate, t' = rot_inv * (-t)
+        ginv[3] = -qfg[3];
+        ginv[4] = -qfg[4];
+        ginv[5] = -qfg[5];
+        ginv[6] = qfg[6];
+        const V3 nt = quat_rot(ginv, V3{-qfg[0], -qfg[1], -qfg[2]});
+        ginv[0] = nt.x;
+        ginv[1] = nt.y;
+        ginv[2] = nt.z;
+        // Obb::from(&aabb): centre = (min+max)*0.5, half = diag*0.5 (obb.rs:19-26); composed with the identity rotation
+        const V3 centre{(bmin[0] + bmax[0]) * 0.5, (bmin[1] + bmax[1]) * 0.5, (bmin[2] + bmax[2]) * 0.5};
+        const V3 sh = quat_rot(ginv, centre);
+        double* q = loc.query_from_obb;
+        q[0] = ginv[0] + sh.x;
+        q[1] = ginv[1] + sh.y;
+        q[2] = ginv[2] + sh.z;
+        q[3] = ginv[3];
+        q[4] = ginv[4];
+        q[5] = ginv[5];
+        q[6] = ginv[6];
+        double* qi = loc.obb_from_query;
+        qi[3] = -q[3];
+        qi[4] = -q[4];
+        qi[5] = -q[5];
+        qi[6] = q[6];
+        const V3 it = quat_rot(qi, V3{-q[0], -q[1], -q[2]});
+        qi[0] = it.x;
+        qi[1] = it.y;
+        qi[2] = it.z;
+        for (int a = 0; a < 3; ++a) loc.half_extent[a] = (bmax[a] - bmin[a]) * 0.5;
+    } else {
+        loc.kind = PCV_LOC_AABB;
+        for (int a = 0; a < 3; ++a) {
+            loc.aabb_min[a] = bmin[a];
+            loc.aabb_max[a] = bmax[a];
+        }
+    }
+    return loc;
+}
+
 // 4x4 inverse by cofactors (the formula nalgebra's try_inverse uses for 4x4); false if det == 0.
 inline bool mat4_try_inverse(const double* m, double* out) {
     double inv[16];

@@ -24,6 +24,7 @@
 #include "kernels_shard.cuh"
 #include "query.cuh"
 #include "xray_pyramid.cuh"
+#include "xray_dir_plan.h"
 #include "s2.cuh"
 #include "synth.cuh"
 
@@ -563,44 +564,13 @@ int pcv_octree_load_dir(pcv_ctx* c, const char* dir, pcv_octree** out) {
     int version = 0;
     if (!decode_meta(buf, h, pn, version))
         return fail(PCV_ERR_INVALID, "meta.pb: unsupported or malformed (version %d; only 13 is read)", version);
-    std::sort(pn.begin(), pn.end(), [](const ParsedNode& a, const ParsedNode& b) { return a.hi != b.hi ? a.hi < b.hi : a.lo < b.lo; });
     pcv_octree* o = new pcv_octree();
     o->ctx = c;
     o->resolution = h.resolution;
-    for (int a = 0; a < 3; ++a) {
-        o->bbox_min[a] = std::fmin(h.bbox_min[a], h.bbox_max[a]);
-        o->bbox_max[a] = std::fmax(h.bbox_min[a], h.bbox_max[a]);
-    }
-    const double E = std::fmax(std::fmax(o->bbox_max[0] - o->bbox_min[0], o->bbox_max[1] - o->bbox_min[1]), o->bbox_max[2] - o->bbox_min[2]);
     uint64_t poff = 0, boff = 0;
-    for (const auto& p : pn) {
-        pcv_node_meta m{};
-        m.id_high = p.hi;
-        m.id_low = p.lo;
-        m.num_points = p.num_points;
-        m.position_encoding = p.enc;
-        if (p.enc < 1 || p.enc > 4) {
-            delete o;
-            return fail(PCV_ERR_INVALID, "Proto: PositionEncoding is invalid");
-        }
-        const u128 id = ((u128)p.hi << 64) | p.lo;
-        m.level = (int)(id >> 120);
-        double e = E, mn[3] = {o->bbox_min[0], o->bbox_min[1], o->bbox_min[2]};
-        for (int lvl = m.level - 1; lvl >= 0; --lvl) {  // node.rs:157-172
-            e /= 2.;
-            const unsigned ci = (unsigned)((id >> (3 * lvl)) & 7);
-            mn[0] += (double)((ci >> 2) & 1) * e;
-            mn[1] += (double)((ci >> 1) & 1) * e;
-            mn[2] += (double)(ci & 1) * e;
-        }
-        for (int a = 0; a < 3; ++a) m.cube_min[a] = mn[a];
-        m.cube_edge = e;
-        boff = (boff + 15) & ~15ull;
-        m.point_offset = poff;
-        m.xyz_byte_offset = boff;
-        poff += (uint64_t)p.num_points;
-        boff += (uint64_t)p.num_points * 3 * (uint64_t)enc_bytes(p.enc);
-        o->nodes.push_back(m);
+    if (!octree_nodes_from_meta(h, std::move(pn), o->bbox_min, o->bbox_max, o->nodes, poff, boff)) {
+        delete o;
+        return fail(PCV_ERR_INVALID, "Proto: PositionEncoding is invalid");
     }
     o->n = poff;
     o->xyz_bytes = boff;
@@ -692,6 +662,7 @@ int pcv_synth_bbox(int kind, double bbox_min[3], double bbox_max[3], double* res
 
 #include "query_api.inl"
 #include "xray_api.inl"
+#include "xray_dir.inl"
 #include "s2_api.inl"
 #include "ply_api.inl"
 #include "shard_api.inl"

@@ -818,12 +818,31 @@ struct XrayOccupyArgs {
     uint32_t ncand;
     uint32_t* hit;            // [ncand]
 };
-__device__ __forceinline__ void xray_cell_range(double v, double v0, double edge, double margin, uint64_t cells, int64_t& lo, int64_t& hi) {
+__host__ __device__ __forceinline__ void xray_cell_range(double v, double v0, double edge, double margin, uint64_t cells, int64_t& lo, int64_t& hi) {
     const double a = floor((v - margin - v0) / edge), b = floor((v + margin - v0) / edge);
     lo = 1, hi = 0;  // empty
     if (!(a == a) || !(b == b) || b < 0.0 || a >= (double)cells) return;
     lo = a < 0.0 ? 0 : (int64_t)a;
     hi = b >= (double)cells ? (int64_t)cells - 1 : (int64_t)b;
+}
+// The per-point arithmetic of the pruning, shared by k_xray_occupy and k_xray_occupy_cells: the decoded point p (global frame)
+// moved into the quadtree's frame like k_xray_bin moves it, then the cells [x0, x1] x [y0, y1] of the level's grid (`cells`
+// per side, cell `edge`, origin (gx, gy)) whose cell widened by `margin` contains it - at most 2 x 2 of them.
+__host__ __device__ __forceinline__ void xray_point_cells(const double p_in[3], const double* qfg, double gx, double gy, double edge, double margin,
+                                                          uint64_t cells, int64_t& x0, int64_t& x1, int64_t& y0, int64_t& y1) {
+    double p[2] = {p_in[0], p_in[1]};
+    if (qfg) {
+        const V3 q = iso_apply(qfg, V3{p_in[0], p_in[1], p_in[2]});
+        p[0] = q.x, p[1] = q.y;
+    }
+    xray_cell_range(p[0], gx, edge, margin, cells, x0, x1);
+    xray_cell_range(p[1], gy, edge, margin, cells, y0, y1);
+}
+// quadtree child k: bit 1 -> +x, bit 0 -> +y (quadtree lib.rs:84-101): the index of cell (ix, iy) of a level
+__host__ __device__ __forceinline__ uint64_t xray_quad_index(uint64_t ix, uint64_t iy, uint32_t level) {
+    uint64_t idx = 0;
+    for (uint32_t b = 0; b < level; ++b) idx |= (((ix >> b) & 1ull) << (2 * b + 1)) | (((iy >> b) & 1ull) << (2 * b));
+    return idx;
 }
 __global__ void __launch_bounds__(256) k_xray_occupy(const __grid_constant__ XrayOccupyArgs a) {
     const uint64_t cells = 1ull << a.level;
@@ -836,17 +855,11 @@ __global__ void __launch_bounds__(256) k_xray_occupy(const __grid_constant__ Xra
             double p[3];
 #pragma unroll
             for (int k = 0; k < 3; ++k) p[k] = decode1_fast(load_code(s + k * bpc, nd.enc), nd.m[k], nd.e, nd.enc);
-            if (a.has_q) {
-                const V3 q = iso_apply(a.query_from_global, V3{p[0], p[1], p[2]});
-                p[0] = q.x, p[1] = q.y;
-            }
             int64_t x0, x1, y0, y1;
-            xray_cell_range(p[0], a.x0, a.edge, a.margin, cells, x0, x1);
-            xray_cell_range(p[1], a.y0, a.edge, a.margin, cells, y0, y1);
+            xray_point_cells(p, a.has_q ? a.query_from_global : nullptr, a.x0, a.y0, a.edge, a.margin, cells, x0, x1, y0, y1);
             for (int64_t ix = x0; ix <= x1; ++ix)
                 for (int64_t iy = y0; iy <= y1; ++iy) {
-                    uint64_t idx = 0;  // quadtree child k: bit 1 -> +x, bit 0 -> +y (quadtree lib.rs:84-101)
-                    for (uint32_t b = 0; b < a.level; ++b) idx |= ((((uint64_t)ix >> b) & 1ull) << (2 * b + 1)) | ((((uint64_t)iy >> b) & 1ull) << (2 * b));
+                    const uint64_t idx = xray_quad_index((uint64_t)ix, (uint64_t)iy, a.level);
                     uint32_t l = 0, h = a.ncand;
                     while (l < h) {
                         const uint32_t m = (l + h) >> 1;
@@ -856,6 +869,68 @@ __global__ void __launch_bounds__(256) k_xray_occupy(const __grid_constant__ Xra
                             h = m;
                     }
                     if (l < a.ncand && a.cand[l] == idx && !a.hit[l]) a.hit[l] = 1;
+                }
+        }
+    }
+}
+// The occupancy pass of the X-ray quadtree built from an on-disk octree (xray_dir.inl): one chunk of node files streamed
+// through the device, every point marking the cells of one level (the leaves) exactly as k_xray_occupy marks candidates,
+// into an open-addressing set of cell indices.  Only cells in [lo, hi] (the sub-root's subtree) are kept.  Index ~0 is the
+// empty slot, so that one cell raises `last` instead; a set that is full raises `overflow` (the host empties it and runs the
+// chunk again: inserting is idempotent).
+struct XrayOccupyCellsArgs {
+    const QNode* nodes;       // the chunk's nodes: cube, encoding, point count, offset of their positions in `xyz`
+    const QTile* tiles;
+    const uint8_t* xyz;
+    uint32_t ntiles;
+    double query_from_global[7];
+    int has_q;
+    double x0, y0, edge, margin;
+    uint32_t level;
+    unsigned long long lo, hi;
+    unsigned long long* set;  // [mask + 1], ~0 = empty
+    uint32_t mask;
+    unsigned int* count;      // slots taken
+    int* overflow;
+    int* last;
+};
+__device__ __forceinline__ void occupy_insert(const XrayOccupyCellsArgs& a, unsigned long long key) {
+    if (key == ~0ull) {
+        *a.last = 1;
+        return;
+    }
+    uint32_t h = (uint32_t)((key * 0x9E3779B97F4A7C15ull) >> 32) & a.mask;
+    for (uint32_t probe = 0; probe <= a.mask; ++probe, h = (h + 1) & a.mask) {
+        const unsigned long long cur = *(volatile unsigned long long*)(a.set + h);
+        if (cur == key) return;
+        if (cur == ~0ull) {
+            const unsigned long long prev = atomicCAS(a.set + h, ~0ull, key);
+            if (prev == ~0ull) {
+                atomicAdd(a.count, 1u);
+                return;
+            }
+            if (prev == key) return;
+        }
+    }
+    *a.overflow = 1;
+}
+__global__ void __launch_bounds__(256) k_xray_occupy_cells(const __grid_constant__ XrayOccupyCellsArgs a) {
+    const uint64_t cells = 1ull << a.level;
+    for (uint32_t ti = blockIdx.x; ti < a.ntiles; ti += gridDim.x) {
+        const QTile t = a.tiles[ti];
+        const QNode nd = a.nodes[t.node];
+        const int bpc = enc_bytes(nd.enc);
+        for (uint32_t i = threadIdx.x; i < t.count; i += blockDim.x) {
+            const uint8_t* s = a.xyz + nd.xyz_off + (uint64_t)(t.first + i) * 3 * bpc;
+            double p[3];
+#pragma unroll
+            for (int k = 0; k < 3; ++k) p[k] = decode1_fast(load_code(s + k * bpc, nd.enc), nd.m[k], nd.e, nd.enc);
+            int64_t x0, x1, y0, y1;
+            xray_point_cells(p, a.has_q ? a.query_from_global : nullptr, a.x0, a.y0, a.edge, a.margin, cells, x0, x1, y0, y1);
+            for (int64_t ix = x0; ix <= x1; ++ix)
+                for (int64_t iy = y0; iy <= y1; ++iy) {
+                    const uint64_t idx = xray_quad_index((uint64_t)ix, (uint64_t)iy, a.level);
+                    if (idx >= a.lo && idx <= a.hi) occupy_insert(a, idx);
                 }
         }
     }

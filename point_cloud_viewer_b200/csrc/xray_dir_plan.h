@@ -1,0 +1,186 @@
+// xray_dir_plan.h — host-only planning of the X-ray quadtree built straight from an on-disk octree (xray_dir.inl; no CUDA:
+// the CPU tests compile it with g++).
+//   octree_nodes_from_meta: meta.pb's nodes -> the node table pcv_octree_load_dir builds (no node file is read)
+//   octree_children:        the 8 children of every node in that table
+//   xray_window:            the nodes a block of leaves can meet: descend from the octree root while the SAT test is not Out
+//   xray_window_size:       what one window takes in device memory (arrays, query tables, the attribute pass flags)
+//   xray_block_location:    a block's location, widened by the pruning margin
+//   xray_select_share:      the budget's share for the node selection (the bounded driver's split)
+//   xray_dir_block_depth:   the block depth from the budget, the images and the largest window of the occupied blocks
+#pragma once
+#include <algorithm>
+#include <cstdint>
+#include <functional>
+#include <vector>
+
+#include "chain.h"
+#include "disk_io.hpp"
+#include "geometry_host.hpp"
+#include "xray_plan.h"
+#include "xray_pyramid.h"
+
+namespace pcv {
+
+// The node table of an octree directory as pcv_octree_load_dir lays it out: sorted by NodeId, cubes from the bounding cube
+// (node.rs:157-172), points node-contiguous, every node's positions 16-byte aligned.  False: an invalid position encoding.
+inline bool octree_nodes_from_meta(const MetaHeader& h, std::vector<ParsedNode> pn, double bmin[3], double bmax[3], std::vector<pcv_node_meta>& nodes,
+                                   uint64_t& npoints, uint64_t& xyz_bytes) {
+    typedef unsigned __int128 id128;
+    std::sort(pn.begin(), pn.end(), [](const ParsedNode& a, const ParsedNode& b) { return a.hi != b.hi ? a.hi < b.hi : a.lo < b.lo; });
+    for (int a = 0; a < 3; ++a) {
+        bmin[a] = std::fmin(h.bbox_min[a], h.bbox_max[a]);
+        bmax[a] = std::fmax(h.bbox_min[a], h.bbox_max[a]);
+    }
+    const double E = std::fmax(std::fmax(bmax[0] - bmin[0], bmax[1] - bmin[1]), bmax[2] - bmin[2]);
+    uint64_t poff = 0, boff = 0;
+    nodes.clear();
+    nodes.reserve(pn.size());
+    for (const auto& p : pn) {
+        pcv_node_meta m{};
+        m.id_high = p.hi;
+        m.id_low = p.lo;
+        m.num_points = p.num_points;
+        m.position_encoding = p.enc;
+        if (p.enc < 1 || p.enc > 4) return false;
+        const id128 id = ((id128)p.hi << 64) | p.lo;
+        m.level = (int)(id >> 120);
+        double e = E, mn[3] = {bmin[0], bmin[1], bmin[2]};
+        for (int lvl = m.level - 1; lvl >= 0; --lvl) {  // node.rs:157-172
+            e /= 2.;
+            const unsigned ci = (unsigned)((id >> (3 * lvl)) & 7);
+            mn[0] += (double)((ci >> 2) & 1) * e;
+            mn[1] += (double)((ci >> 1) & 1) * e;
+            mn[2] += (double)(ci & 1) * e;
+        }
+        for (int a = 0; a < 3; ++a) m.cube_min[a] = mn[a];
+        m.cube_edge = e;
+        boff = (boff + 15) & ~15ull;
+        m.point_offset = poff;
+        m.xyz_byte_offset = boff;
+        poff += (uint64_t)p.num_points;
+        boff += (uint64_t)p.num_points * 3 * (uint64_t)enc_bytes(p.enc);
+        nodes.push_back(m);
+    }
+    npoints = poff;
+    xyz_bytes = boff;
+    return true;
+}
+
+// children[8 i + k]: index of child k of node i in `nodes` (sorted by NodeId), -1 if absent.
+inline std::vector<int32_t> octree_children(const std::vector<pcv_node_meta>& nodes) {
+    typedef unsigned __int128 id128;
+    std::vector<int32_t> ch(nodes.size() * 8, -1);
+    auto find = [&](uint64_t hi, uint64_t lo) -> int64_t {
+        auto it = std::lower_bound(nodes.begin(), nodes.end(), std::make_pair(hi, lo),
+                                   [](const pcv_node_meta& m, const std::pair<uint64_t, uint64_t>& k) { return m.id_high != k.first ? m.id_high < k.first : m.id_low < k.second; });
+        return it != nodes.end() && it->id_high == hi && it->id_low == lo ? (int64_t)(it - nodes.begin()) : -1;
+    };
+    for (size_t i = 0; i < nodes.size(); ++i) {
+        if (nodes[i].level == 0) continue;
+        const id128 id = ((id128)nodes[i].id_high << 64) | nodes[i].id_low;
+        const id128 idx = id & ((((id128)1) << 120) - 1);
+        const id128 pid = ((id128)(nodes[i].level - 1) << 120) | (idx >> 3);  // node.rs:136-144
+        const int64_t p = find((uint64_t)(pid >> 64), (uint64_t)pid);
+        if (p >= 0) ch[(size_t)p * 8 + (size_t)(idx & 7)] = (int32_t)i;
+    }
+    return ch;
+}
+
+// sat() of sat.rs:174-194 with A = the location and B = the node cube (min m, edge e): sat_cube of query.cuh on the host.
+inline bool sat_cube_out(const QueryGeom& g, const double m[3], double e) {
+    if (g.kind == PCV_LOC_ALL) return false;
+    const double mx[3] = {m[0] + e, m[1] + e, m[2] + e};
+    for (int k = 0; k < g.naxes; ++k) {
+        const double* ax = g.axes[k];
+        double alo = 1.7976931348623157e308, ahi = -1.7976931348623157e308, blo = alo, bhi = ahi;
+        for (int i = 0; i < 8; ++i) {
+            const double pa = g.corners[i][0] * ax[0] + g.corners[i][1] * ax[1] + g.corners[i][2] * ax[2];
+            alo = std::fmin(alo, pa);
+            ahi = std::fmax(ahi, pa);
+            const double cx = (i & 1) ? mx[0] : m[0], cy = (i & 2) ? mx[1] : m[1], cz = (i & 4) ? mx[2] : m[2];
+            const double pb = cx * ax[0] + cy * ax[1] + cz * ax[2];
+            blo = std::fmin(blo, pb);
+            bhi = std::fmax(bhi, pb);
+        }
+        if (blo > ahi || bhi < alo) return true;
+    }
+    return false;
+}
+
+// The window of a location: every node whose cube and whose ancestors' cubes are not Out, found by descending from the root
+// (nodes_in_location's BFS semantics).  Sorted node indices, closed under ancestors: a valid octree on its own.
+inline std::vector<uint32_t> xray_window(const std::vector<pcv_node_meta>& nodes, const std::vector<int32_t>& children, const QueryGeom& g) {
+    std::vector<uint32_t> out, stack;
+    if (nodes.empty() || nodes[0].level != 0) return out;
+    stack.push_back(0);
+    while (!stack.empty()) {
+        const uint32_t i = stack.back();
+        stack.pop_back();
+        if (sat_cube_out(g, nodes[i].cube_min, nodes[i].cube_edge)) continue;
+        out.push_back(i);
+        for (int k = 0; k < 8; ++k)
+            if (children[(size_t)i * 8 + k] >= 0) stack.push_back((uint32_t)children[(size_t)i * 8 + k]);
+    }
+    std::sort(out.begin(), out.end());
+    return out;
+}
+
+// Device bytes per window node besides its points: the query node (64 bytes), its 8 children (32), the attribute strategies'
+// relation and pass flags (2).
+constexpr uint64_t kWindowNodeBytes = 64 + 32 + 2;
+struct WindowSize {
+    uint64_t bytes = 0, points = 0, xyz_bytes = 0;
+};
+// What one window takes on the device: its positions laid out as load_dir lays them (16-byte aligned, + 32 bytes of slack for
+// the kernels' 16-byte staging), colours, intensities if the directory has them, and the per-node tables.
+inline WindowSize xray_window_size(const std::vector<pcv_node_meta>& nodes, const std::vector<uint32_t>& win, bool has_intensity) {
+    WindowSize s;
+    for (uint32_t i : win) {
+        s.xyz_bytes = (s.xyz_bytes + 15) & ~15ull;
+        s.xyz_bytes += (uint64_t)nodes[i].num_points * 3 * (uint64_t)enc_bytes(nodes[i].position_encoding);
+        s.points += (uint64_t)nodes[i].num_points;
+    }
+    s.bytes = s.xyz_bytes + 32 + std::max<uint64_t>(3 * s.points, 16) + (has_intensity ? 4 * s.points : 0) + kWindowNodeBytes * win.size();
+    return s;
+}
+
+// The location of block `bidx` at quadtree level B: its rect (the quad_rect_of recurrence) over the z range of the box, every
+// side widened by `margin`, as an Aabb or, under query_from_global, the Obb xray_location builds for a leaf.  A leaf's rect comes
+// from the same recurrence, so it lies within a few ulps of its block's rect; the margin is far above that.
+inline pcv_location xray_block_location(const QuadRect& rect, int B, uint64_t bidx, const double bmin[3], const double bmax[3], double margin,
+                                        const double* qfg) {
+    const QuadRect r = quad_rect_of(QuadId{(uint8_t)B, bidx}, rect);
+    const double tmin[3] = {r.min_x - margin, r.min_y - margin, bmin[2] - margin};
+    const double tmax[3] = {r.min_x + r.edge + margin, r.min_y + r.edge + margin, bmax[2] + margin};
+    return xray_location(tmin, tmax, qfg);
+}
+
+// The bounded driver's split of what the budget leaves after `fixed`: an eighth for the node selection (frontier capacity
+// `sel_cap` pairs and `max_loc` locations per selection), the rest for the block's images and a key batch.
+struct XraySelectShare {
+    uint64_t sel_bytes = 0, max_loc = 0;
+    uint32_t sel_cap = 0;
+};
+inline XraySelectShare xray_select_share(uint64_t budget, uint64_t fixed, uint64_t per_loc) {
+    XraySelectShare s;
+    s.sel_bytes = budget > fixed ? (budget - fixed) / 8 : 0;
+    s.sel_cap = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(s.sel_bytes / 2 / 40, 64), 48ull << 20);
+    s.max_loc = std::max<uint64_t>(1, s.sel_bytes / 2 / per_loc);
+    return s;
+}
+
+// Block depth g of the directory driver: the largest g <= g_max for which the block images, the node selection and the
+// largest window over the occupied blocks at level deepest - g (`window_max(g)`, UINT64_MAX: a window too large to hold) fit
+// the budget besides `fixed`.  A smaller g means a deeper block level and smaller windows.  -1: not even g = 0 fits.
+inline int xray_dir_block_depth(uint64_t budget, uint64_t fixed, int depth, int g_max, uint64_t leaf_bytes, uint64_t tile_bytes, uint64_t per_loc,
+                                const std::function<uint64_t(int)>& window_max) {
+    for (int g = g_max; g >= 0; --g) {
+        const uint64_t w = window_max(g);
+        if (w == UINT64_MAX || fixed + w >= budget) continue;
+        const XraySelectShare s = xray_select_share(budget, fixed + w, per_loc);
+        if (xray_block_depth(budget, fixed + w + s.sel_bytes + 40ull * s.sel_cap, depth, g, leaf_bytes, tile_bytes) >= g) return g;
+    }
+    return -1;
+}
+
+}  // namespace pcv
