@@ -306,6 +306,44 @@ int pcv_xray_quadtree_from_dir_write_dir(pcv_ctx* ctx, const char* octree_dir, c
                                          const char* out_dir, pcv_xray_quadtree_info* info_out, pcv_xray_bounded_info* bounded_info_out,
                                          pcv_xray_dir_info* dir_info_out);
 
+/* ---- point queries straight from an octree directory (Octree over OnDiskDataProvider, octree/mod.rs:156-215, 337-352) ---- */
+/* A directory-backed octree: open reads meta.pb into the node table pcv_octree_load_dir builds and puts its query tables on the
+ * device; node files are only stat'ed.  Every call reads, uploads and culls only the nodes it selects, in chunks cut at 2048-point
+ * tile boundaries (a node larger than a chunk is read in byte ranges across several chunks), with two pinned host buffers: host
+ * threads read chunk i+1 while the device culls chunk i.  Results equal the same calls over pcv_octree_load_dir of the directory,
+ * except that src_index is the point's slot (point_offset + j of its node in pcv_octree_dir_nodes; load_dir reports 0).
+ * max_device_bytes bounds everything the handle and its calls allocate, the tables included (0: most of the free device memory);
+ * a budget that cannot hold the tables, the selection scratch and one chunk of one tile at the widest encoding fails at open with
+ * PCV_ERR_UNSUPPORTED.  Errors: a meta.pb other than version 13 -> PCV_ERR_INVALID; a missing or wrongly sized .xyz / .rgb file
+ * -> PCV_ERR_NOT_FOUND at open, and from the call that reads a file that has shrunk since.  A handle serialises on its context. */
+typedef struct pcv_octree_dir pcv_octree_dir;
+int pcv_octree_dir_open(pcv_ctx* ctx, const char* dir, uint64_t max_device_bytes, pcv_octree_dir** out);
+void pcv_octree_dir_close(pcv_octree_dir* d);
+int pcv_octree_dir_info(const pcv_octree_dir* d, uint64_t* num_nodes, uint64_t* num_points, uint64_t* xyz_bytes, double* resolution,
+                        double bbox_min[3], double bbox_max[3], int* has_intensity);
+int pcv_octree_dir_nodes(const pcv_octree_dir* d, pcv_node_meta* out, uint64_t cap); /* == pcv_octree_nodes of load_dir */
+/* Selection only: no node file is read. */
+int pcv_octree_dir_nodes_in_location(const pcv_octree_dir* d, const pcv_location* loc, uint64_t* ids_hi_lo, uint64_t cap, uint64_t* n_out);
+int pcv_octree_dir_visible_nodes(const pcv_octree_dir* d, const double clip_from_world[16], uint64_t* ids_hi_lo, uint64_t cap, uint64_t* n_out);
+int pcv_octree_dir_query_points(const pcv_octree_dir* d, const pcv_location* loc, const pcv_interval* filters, uint32_t nfilt,
+                                uint64_t batch_size, pcv_batch_cb cb, void* user);
+/* counts_out / tested_out as pcv_query_batch_device; every node some location visits is read once per call.  A frontier that
+ * does not fit what the budget leaves -> PCV_ERR_UNSUPPORTED ("split the batch"). */
+int pcv_octree_dir_query_batch(const pcv_octree_dir* d, const pcv_location* locs, uint32_t nloc, const pcv_interval* filters,
+                               uint32_t nfilt, uint64_t* counts_out, uint64_t* tested_out);
+/* pcv_nodes_data_blob's reply, read from the node files straight into `out` on the host. */
+int pcv_octree_dir_nodes_data_blob(const pcv_octree_dir* d, const uint64_t* ids_hi_lo, uint32_t num_nodes, void* out, uint64_t cap,
+                                   uint64_t* size_out);
+typedef struct pcv_dir_query_stats {  /* the last call on the handle                                                     */
+    uint64_t max_device_bytes, peak_device_bytes;   /* peak: everything the handle held during the call, tables included */
+    uint64_t chunks, node_files_read, bytes_read, bytes_uploaded;
+    uint64_t visited_pairs, tested_points, returned_points;
+    double ms_select, ms_read_wait, ms_total;       /* wall; ms_read_wait: time the device sat idle waiting for reads    */
+    float ms_cull;                                  /* CUDA events, summed over chunks                                   */
+    uint32_t kernel_launches;
+} pcv_dir_query_stats;
+int pcv_octree_dir_last_stats(const pcv_octree_dir* d, pcv_dir_query_stats* out);
+
 /* ---- f4: the S2-cell point cloud (src/read_write/s2.rs, src/s2_cells/mod.rs, src/geometry/s2_cell_union.rs) ---- */
 /* Cell ids are the S2 library's 64-bit CellID values (face, Hilbert position, level marker bit); the arithmetic is the `s2`
  * crate's, restated (csrc/s2.h): integer and IEEE +, *, /, sqrt only, identical on host and device. */

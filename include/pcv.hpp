@@ -256,6 +256,93 @@ class Octree {
     std::vector<pcv_node_meta> nodes_;
 };
 
+inline PointsBatch batch_from(const pcv_batch* b) {
+    PointsBatch pb;
+    pb.position.resize(b->n);
+    pb.color.resize(b->n);
+    for (uint64_t i = 0; i < b->n; ++i) {
+        pb.position[i] = {b->xyz[3 * i], b->xyz[3 * i + 1], b->xyz[3 * i + 2]};
+        pb.color[i] = {b->rgb[3 * i], b->rgb[3 * i + 1], b->rgb[3 * i + 2]};
+    }
+    if (b->intensity) pb.intensity.assign(b->intensity, b->intensity + b->n);
+    pb.source_index.assign(b->src_index, b->src_index + b->n);
+    return pb;
+}
+
+// An octree directory queried where it lies (Octree over OnDiskDataProvider, octree/mod.rs:156-215, 337-352): the node table is
+// on the device and every query reads only the nodes it selects, within `max_device_bytes`.  Results equal Octree::from_directory's;
+// a batch's source_index is the point's slot in nodes() (point_offset + j of its node).
+class OctreeDir {
+   public:
+    OctreeDir(Context& ctx, const std::string& dir, uint64_t max_device_bytes = 0) {
+        check(pcv_octree_dir_open(ctx.raw(), dir.c_str(), max_device_bytes, &d_));
+        uint64_t nn = 0;
+        check(pcv_octree_dir_info(d_, &nn, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr));
+        nodes_.resize(nn);
+        check(pcv_octree_dir_nodes(d_, nodes_.data(), nn));
+    }
+    OctreeDir(const OctreeDir&) = delete;
+    OctreeDir& operator=(const OctreeDir&) = delete;
+    ~OctreeDir() { pcv_octree_dir_close(d_); }
+    const std::vector<pcv_node_meta>& nodes() const { return nodes_; }
+    std::vector<NodeId> get_visible_nodes(const double projection_matrix[16]) const {
+        std::vector<uint64_t> ids(2 * nodes_.size() + 2);
+        uint64_t n = 0;
+        check(pcv_octree_dir_visible_nodes(d_, projection_matrix, ids.data(), nodes_.size(), &n));
+        return to_ids(ids, n);
+    }
+    std::vector<NodeId> nodes_in_location(const PointLocation& loc) const {
+        std::vector<uint64_t> ids(2 * nodes_.size() + 2);
+        uint64_t n = 0;
+        check(pcv_octree_dir_nodes_in_location(d_, &loc.raw, ids.data(), nodes_.size(), &n));
+        return to_ids(ids, n);
+    }
+    // PointQuery streamed in batches of `batch_size` points (the last one short); func returns false to stop.  Returns true if
+    // every batch was consumed.
+    bool for_each_batch(const PointQuery& query, size_t batch_size, const std::function<bool(PointsBatch&&)>& func) const {
+        auto tramp = [](void* user, const pcv_batch* b) -> int { return (*(const std::function<bool(PointsBatch&&)>*)user)(batch_from(b)) ? 0 : 1; };
+        std::vector<pcv_interval> f;
+        for (auto& iv : query.filter_intervals) f.push_back(pcv_interval{iv.lower_bound, iv.upper_bound});
+        const int rc = pcv_octree_dir_query_points(d_, &query.location.raw, f.empty() ? nullptr : f.data(), (uint32_t)f.size(), batch_size, tramp,
+                                                   (void*)&func);
+        if (rc == PCV_ERR_CANCELLED) return false;
+        check(rc);
+        return true;
+    }
+    // survivors and tested points of every location, each visited node read once
+    void query_batch(const std::vector<PointLocation>& locs, std::vector<uint64_t>& counts, std::vector<uint64_t>& tested) const {
+        std::vector<pcv_location> raw;
+        for (auto& l : locs) raw.push_back(l.raw);
+        counts.assign(locs.size(), 0);
+        tested.assign(locs.size(), 0);
+        check(pcv_octree_dir_query_batch(d_, raw.data(), (uint32_t)raw.size(), nullptr, 0, counts.data(), tested.data()));
+    }
+    std::vector<uint8_t> nodes_data_blob(const std::vector<NodeId>& ids) const {
+        std::vector<uint64_t> hl;
+        for (auto& id : ids) hl.push_back(id.high), hl.push_back(id.low);
+        uint64_t size = 0;
+        check(pcv_octree_dir_nodes_data_blob(d_, hl.data(), (uint32_t)ids.size(), nullptr, 0, &size));
+        std::vector<uint8_t> blob(size);
+        if (size) check(pcv_octree_dir_nodes_data_blob(d_, hl.data(), (uint32_t)ids.size(), blob.data(), size, &size));
+        return blob;
+    }
+    pcv_dir_query_stats last_stats() const {
+        pcv_dir_query_stats s{};
+        check(pcv_octree_dir_last_stats(d_, &s));
+        return s;
+    }
+    pcv_octree_dir* raw() const { return d_; }
+
+   private:
+    static std::vector<NodeId> to_ids(const std::vector<uint64_t>& v, uint64_t n) {
+        std::vector<NodeId> out(n);
+        for (uint64_t i = 0; i < n; ++i) out[i] = NodeId{v[2 * i], v[2 * i + 1]};
+        return out;
+    }
+    pcv_octree_dir* d_ = nullptr;
+    std::vector<pcv_node_meta> nodes_;
+};
+
 // build_octree(output_directory, resolution, bounding_box, input, attributes) — generation.rs:289-295.  `input` is drained on
 // the calling thread; colour is mandatory; attributes selects whether intensity is carried.  Returns the GPU-resident
 // octree as well (the reference returns ()).
@@ -446,16 +533,7 @@ class ParallelIterator {
         } st{&func};
         auto tramp = [](void* user, const pcv_batch* b) -> int {
             State* s = (State*)user;
-            PointsBatch pb;
-            pb.position.resize(b->n);
-            pb.color.resize(b->n);
-            for (uint64_t i = 0; i < b->n; ++i) {
-                pb.position[i] = {b->xyz[3 * i], b->xyz[3 * i + 1], b->xyz[3 * i + 2]};
-                pb.color[i] = {b->rgb[3 * i], b->rgb[3 * i + 1], b->rgb[3 * i + 2]};
-            }
-            if (b->intensity) pb.intensity.assign(b->intensity, b->intensity + b->n);
-            pb.source_index.assign(b->src_index, b->src_index + b->n);
-            return (*s->f)(std::move(pb)) ? 0 : 1;
+            return (*s->f)(batch_from(b)) ? 0 : 1;
         };
         std::vector<pcv_interval> f;
         for (auto& iv : query_.filter_intervals) f.push_back(pcv_interval{iv.lower_bound, iv.upper_bound});

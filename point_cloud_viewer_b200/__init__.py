@@ -204,6 +204,10 @@ class Context:
                                                              os.fsencode(str(out_dir)), C.byref(info), C.byref(binfo), C.byref(dinfo)))
         return _xray_info(info, binfo, dinfo)
 
+    def open_dir(self, directory, max_device_bytes=0):
+        """An OctreeDir over the octree in `directory`: queries read only the nodes they select (0: most of the free memory)."""
+        return OctreeDir(self, directory, max_device_bytes)
+
     def load_dir(self, directory):
         out = C.c_void_p()
         N.check(N.lib().pcv_octree_load_dir(self.h, str(directory).encode(), C.byref(out)))
@@ -584,38 +588,10 @@ class Octree:
     def query_points(self, loc, callback=None, filters=(), batch_size=500000):
         """Streams batches dict(xyz (n,3) f64, rgb (n,3), intensity, src).  A callback returning a truthy
         value cancels the stream (ErrorKind::Channel); without a callback the batches are returned."""
-        f = np.asarray(filters, np.float64).reshape(-1)
-        nf = len(f) // 2
-        got = []
-
-        def tramp(_user, bp):
-            b = bp.contents
-            n = b.n
-            d = dict(
-                xyz=np.ctypeslib.as_array(C.cast(b.xyz, C.POINTER(C.c_double)), (n, 3)).copy() if n else np.zeros((0, 3)),
-                rgb=np.ctypeslib.as_array(C.cast(b.rgb, C.POINTER(C.c_uint8)), (n, 3)).copy() if n else np.zeros((0, 3), np.uint8),
-                intensity=np.ctypeslib.as_array(C.cast(b.intensity, C.POINTER(C.c_float)), (n,)).copy() if (n and b.intensity) else None,
-                src=np.ctypeslib.as_array(C.cast(b.src_index, C.POINTER(C.c_uint64)), (n,)).copy() if n else np.zeros(0, np.uint64),
-            )
-            if callback is None:
-                got.append(d)
-                return 0
-            return 1 if callback(d) else 0
-
-        cb = N.BATCH_CB(tramp)
-        rc = N.lib().pcv_query_points(self.h, C.byref(loc), _p(f) if nf else None, nf, int(batch_size), cb, None)
-        if rc == -5:
-            raise PcvError(rc, "cancelled by callback")
-        N.check(rc)
-        return got
+        return _query_points(N.lib().pcv_query_points, self.h, loc, callback, filters, batch_size)
 
     def query_batch_device(self, locs, filters=()):
-        arr = (N.Location * len(locs))(*locs)
-        f = np.asarray(filters, np.float64).reshape(-1)
-        nf = len(f) // 2
-        counts, tested = np.zeros(len(locs), np.uint64), np.zeros(len(locs), np.uint64)
-        N.check(N.lib().pcv_query_batch_device(self.h, arr, len(locs), _p(f) if nf else None, nf, _p(counts), _p(tested)))
-        return counts, tested
+        return _query_batch(N.lib().pcv_query_batch_device, self.h, locs, filters)
 
     def last_query_stats(self):
         """Timing / traffic of the last query_batch_device call (pcv_query_stats)."""
@@ -684,8 +660,121 @@ class Octree:
         return _xray_info(info, binfo)
 
 
+def _query_points(fn, h, loc, callback, filters, batch_size):
+    f = np.asarray(filters, np.float64).reshape(-1)
+    nf = len(f) // 2
+    got = []
+
+    def tramp(_user, bp):
+        b = bp.contents
+        n = b.n
+        d = dict(
+            xyz=np.ctypeslib.as_array(C.cast(b.xyz, C.POINTER(C.c_double)), (n, 3)).copy() if n else np.zeros((0, 3)),
+            rgb=np.ctypeslib.as_array(C.cast(b.rgb, C.POINTER(C.c_uint8)), (n, 3)).copy() if n else np.zeros((0, 3), np.uint8),
+            intensity=np.ctypeslib.as_array(C.cast(b.intensity, C.POINTER(C.c_float)), (n,)).copy() if (n and b.intensity) else None,
+            src=np.ctypeslib.as_array(C.cast(b.src_index, C.POINTER(C.c_uint64)), (n,)).copy() if n else np.zeros(0, np.uint64),
+        )
+        if callback is None:
+            got.append(d)
+            return 0
+        return 1 if callback(d) else 0
+
+    cb = N.BATCH_CB(tramp)
+    rc = fn(h, C.byref(loc), _p(f) if nf else None, nf, int(batch_size), cb, None)
+    if rc == -5:
+        raise PcvError(rc, "cancelled by callback")
+    N.check(rc)
+    return got
+
+
+def _query_batch(fn, h, locs, filters):
+    arr = (N.Location * len(locs))(*locs)
+    f = np.asarray(filters, np.float64).reshape(-1)
+    nf = len(f) // 2
+    counts, tested = np.zeros(len(locs), np.uint64), np.zeros(len(locs), np.uint64)
+    N.check(fn(h, arr, len(locs), _p(f) if nf else None, nf, _p(counts), _p(tested)))
+    return counts, tested
+
+
+class OctreeDir:
+    """An octree directory queried where it lies (pcv_octree_dir): the node table and its query tables are on the device, and
+    every query reads, uploads and culls only the nodes it selects, in chunks, within `max_device_bytes`.  The methods have the
+    shapes of Octree's; query_points' `src` is the point's slot (point_offset + j of its node in `meta`)."""
+
+    def __init__(self, ctx, directory, max_device_bytes=0):
+        self.ctx = ctx
+        self.h = None
+        h = C.c_void_p()
+        N.check(N.lib().pcv_octree_dir_open(ctx.h, os.fsencode(str(directory)), int(max_device_bytes), C.byref(h)))
+        self.h = h
+        nn, npts, xb, res = C.c_uint64(), C.c_uint64(), C.c_uint64(), C.c_double()
+        mn, mx, hi = (C.c_double * 3)(), (C.c_double * 3)(), C.c_int()
+        N.check(N.lib().pcv_octree_dir_info(self.h, C.byref(nn), C.byref(npts), C.byref(xb), C.byref(res), mn, mx, C.byref(hi)))
+        self.num_nodes, self.num_points, self.xyz_bytes, self.resolution = nn.value, npts.value, xb.value, res.value
+        self.bbox_min, self.bbox_max, self.has_intensity = np.array(mn), np.array(mx), bool(hi.value)
+        arr = (N.NodeMeta * max(nn.value, 1))()
+        N.check(N.lib().pcv_octree_dir_nodes(self.h, arr, nn.value))
+        self.meta = np.frombuffer(arr, dtype=NODE_DTYPE, count=nn.value).copy() if nn.value else np.zeros(0, NODE_DTYPE)
+
+    def nodes(self):
+        """The node table, as Octree.meta of load_dir (structured array of NODE_DTYPE)."""
+        return self.meta
+
+    def close(self):
+        if self.h and self.ctx.h:
+            N.lib().pcv_octree_dir_close(self.h)
+        self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def nodes_in_location(self, loc):
+        cap = self.num_nodes + 1
+        out = np.zeros(2 * cap, np.uint64)
+        n = C.c_uint64()
+        N.check(N.lib().pcv_octree_dir_nodes_in_location(self.h, C.byref(loc), _p(out), cap, C.byref(n)))
+        return [node_name(out[2 * i], out[2 * i + 1]) for i in range(n.value)]
+
+    def get_visible_nodes(self, clip_from_world):
+        m = np.asarray(clip_from_world, np.float64)
+        flat = m.T.reshape(-1) if m.ndim == 2 else m
+        cap = self.num_nodes + 1
+        out = np.zeros(2 * cap, np.uint64)
+        n = C.c_uint64()
+        N.check(N.lib().pcv_octree_dir_visible_nodes(self.h, (C.c_double * 16)(*[float(v) for v in flat]), _p(out), cap, C.byref(n)))
+        return [node_name(out[2 * i], out[2 * i + 1]) for i in range(n.value)]
+
+    def query_points(self, loc, callback=None, filters=(), batch_size=500000):
+        """Octree.query_points over the directory; `src` holds every point's slot."""
+        return _query_points(N.lib().pcv_octree_dir_query_points, self.h, loc, callback, filters, batch_size)
+
+    def query_batch(self, locs, filters=()):
+        """(counts, tested) of Octree.query_batch_device, every visited node read once."""
+        return _query_batch(N.lib().pcv_octree_dir_query_batch, self.h, locs, filters)
+
+    def nodes_data_blob(self, names, out=None):
+        ids = np.zeros(2 * len(names), np.uint64)
+        for k, nm in enumerate(names):
+            ids[2 * k], ids[2 * k + 1] = node_id_from_name(nm)
+        size = C.c_uint64()
+        N.check(N.lib().pcv_octree_dir_nodes_data_blob(self.h, _p(ids), len(names), None, 0, C.byref(size)))
+        if out is None:
+            out = np.zeros(max(size.value, 1), np.uint8)
+        N.check(N.lib().pcv_octree_dir_nodes_data_blob(self.h, _p(ids), len(names), _p(out), out.nbytes if hasattr(out, "nbytes") else len(out), C.byref(size)))
+        return out[: size.value]
+
+    def last_stats(self):
+        """pcv_dir_query_stats of the last call on the handle."""
+        st = N.DirQueryStats()
+        N.check(N.lib().pcv_octree_dir_last_stats(self.h, C.byref(st)))
+        return {k: getattr(st, k) for k, _ in N.DirQueryStats._fields_}
+
+
 class S2Cloud:
-    """pcv_s2cloud: the S2-cell point cloud (S2Cells / S2Meta of src/s2_cells/mod.rs) resident in HBM."""
+    """pcv_s2cloud:the S2-cell point cloud (S2Cells / S2Meta of src/s2_cells/mod.rs) resident in HBM."""
 
     def __init__(self, ctx, handle):
         self.ctx, self.h = ctx, handle

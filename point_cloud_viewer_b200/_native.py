@@ -140,6 +140,15 @@ class XrayDirInfo(C.Structure):
                 ("largest_window_points", C.c_uint64), ("occupied_leaves", C.c_uint64), ("ms_occupancy", C.c_double), ("ms_windows", C.c_double)]
 
 
+class DirQueryStats(C.Structure):
+    """pcv_dir_query_stats (include/pcv.h)."""
+
+    _fields_ = [("max_device_bytes", C.c_uint64), ("peak_device_bytes", C.c_uint64), ("chunks", C.c_uint64), ("node_files_read", C.c_uint64),
+                ("bytes_read", C.c_uint64), ("bytes_uploaded", C.c_uint64), ("visited_pairs", C.c_uint64), ("tested_points", C.c_uint64),
+                ("returned_points", C.c_uint64), ("ms_select", C.c_double), ("ms_read_wait", C.c_double), ("ms_total", C.c_double), ("ms_cull", C.c_float),
+                ("kernel_launches", C.c_uint32)]
+
+
 XRAY_TILE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint8, C.c_uint64, C.POINTER(C.c_uint8), C.c_uint32)
 
 
@@ -216,6 +225,16 @@ SYMBOLS = [
                                              C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo), C.POINTER(XrayDirInfo)]),
     ("pcv_xray_quadtree_from_dir_write_dir", C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(XrayQuadtreeParams), C.c_uint64, C.c_char_p,
                                                        C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo), C.POINTER(XrayDirInfo)]),
+    ("pcv_octree_dir_open", C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, C.POINTER(C.c_void_p)]),
+    ("pcv_octree_dir_close", None, [C.c_void_p]),
+    ("pcv_octree_dir_info", C.c_int, [C.c_void_p, _u64p, _u64p, _u64p, _dp, _dp, _dp, C.POINTER(C.c_int)]),
+    ("pcv_octree_dir_nodes", C.c_int, [C.c_void_p, C.POINTER(NodeMeta), C.c_uint64]),
+    ("pcv_octree_dir_nodes_in_location", C.c_int, [C.c_void_p, C.POINTER(Location), C.c_void_p, C.c_uint64, _u64p]),
+    ("pcv_octree_dir_visible_nodes", C.c_int, [C.c_void_p, _dp, C.c_void_p, C.c_uint64, _u64p]),
+    ("pcv_octree_dir_query_points", C.c_int, [C.c_void_p, C.POINTER(Location), C.c_void_p, C.c_uint32, C.c_uint64, BATCH_CB, C.c_void_p]),
+    ("pcv_octree_dir_query_batch", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
+    ("pcv_octree_dir_nodes_data_blob", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, _u64p]),
+    ("pcv_octree_dir_last_stats", C.c_int, [C.c_void_p, C.POINTER(DirQueryStats)]),
     ("pcv_s2_cell_ids", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_uint32, C.c_void_p]),
     ("pcv_s2_build", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_uint32, C.POINTER(C.c_void_p)]),
     ("pcv_s2_build_device", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_uint32, C.POINTER(C.c_void_p)]),

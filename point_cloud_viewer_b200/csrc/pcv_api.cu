@@ -16,6 +16,7 @@
 #include <thread>
 
 #include "../../include/pcv.h"
+#include "dir_query_plan.h"
 #include "disk_io.hpp"
 #include "octree_obj.hpp"
 #include "ooc_plan.h"
@@ -662,7 +663,9 @@ int pcv_synth_bbox(int kind, double bbox_min[3], double bbox_max[3], double* res
 
 #include "query_api.inl"
 #include "xray_api.inl"
+#include "dir_octree.inl"
 #include "xray_dir.inl"
+#include "dir_query.inl"
 #include "s2_api.inl"
 #include "ply_api.inl"
 #include "shard_api.inl"

@@ -247,8 +247,11 @@ __device__ __forceinline__ bool eval_point(const CullArgs& a, const QueryGeom& g
     return keep;
 }
 
-template <bool WRITE>
-__global__ void __launch_bounds__(256) k_cull(const __grid_constant__ CullArgs a) {
+// The ordered cull of one tile per block: count pass (WRITE = false), then after k_scan_u32 the write pass.  SLOT = false: the
+// survivor's provenance is gathered from the resident `src` array (k_cull); SLOT = true: it is the point's slot in the node table,
+// slot_base[piece] + first + i (k_cull_chunk, for pieces of nodes streamed from disk).
+template <bool WRITE, bool SLOT>
+__device__ __forceinline__ void cull_tile(const CullArgs& a, const uint64_t* slot_base, uint64_t* out_slot) {
     __shared__ uint32_t warp_cnt[8];
     __shared__ uint32_t running;
     const QTile t = a.tiles[blockIdx.x];
@@ -282,13 +285,30 @@ __global__ void __launch_bounds__(256) k_cull(const __grid_constant__ CullArgs a
             a.out_rgb[3 * dst + 1] = a.rgb[3 * sp + 1];
             a.out_rgb[3 * dst + 2] = a.rgb[3 * sp + 2];
             if (a.out_intensity) a.out_intensity[dst] = a.intensity[sp];
-            a.out_src[dst] = a.src[sp];
+            if (SLOT)
+                out_slot[dst] = slot_base[t.node] + t.first + i;
+            else
+                a.out_src[dst] = a.src[sp];
         }
         __syncthreads();
         if (threadIdx.x == 0) running += total;
         __syncthreads();
     }
     if (!WRITE && threadIdx.x == 0) a.tile_keep[blockIdx.x] = running;
+}
+template <bool WRITE>
+__global__ void __launch_bounds__(256) k_cull(const __grid_constant__ CullArgs a) {
+    cull_tile<WRITE, false>(a, nullptr, nullptr);
+}
+// One chunk of a directory-backed query: `nodes` / `tiles` are the chunk's pieces (chunk-local offsets), `src` / `out_src` unused.
+struct CullChunkArgs {
+    CullArgs c;
+    const uint64_t* slot_base;  // [piece] point_offset of the piece's node + the piece's first point
+    uint64_t* out_slot;
+};
+template <bool WRITE>
+__global__ void __launch_bounds__(256) k_cull_chunk(const __grid_constant__ CullChunkArgs a) {
+    cull_tile<WRITE, true>(a.c, a.slot_base, a.out_slot);
 }
 
 // Exclusive scan of n u32 values in place; total (u64) to *total_out.  Single block; n is at most a few million tiles.
@@ -598,6 +618,55 @@ __global__ void __launch_bounds__(256) k_cull_fused(const __grid_constant__ Cull
             __syncthreads();  // the staging arrays and wcnt are reused by the next round
         }
         if (threadIdx.x == 0 && kept_tile) atomicAdd(&f.kept[t.loc], (unsigned long long)kept_tile);
+        __syncthreads();  // sxyz is reused by the next tile
+    }
+}
+
+// The per-location count of k_cull_fused over one chunk of a directory-backed batched query: the work list holds one tile per
+// kQueryTile points of every (location, piece) pair, the positions are staged as in k_cull_fused, survivors are counted with
+// ballots and added to kept[loc] with one atomic per tile.  Nothing is stored.
+__global__ void __launch_bounds__(256) k_cull_count_chunk(const __grid_constant__ CullArgs a, uint32_t ntiles, unsigned long long* __restrict__ kept) {
+    __shared__ __align__(16) uint8_t sxyz[kCullStage];
+    __shared__ uint32_t wcnt[8];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (uint32_t ti = blockIdx.x; ti < ntiles; ti += gridDim.x) {
+        const QTile t = a.tiles[ti];
+        const QueryGeom& g = a.geoms[t.loc];
+        const QNode nd = a.nodes[t.node];
+        const bool staged = nd.enc != ENC_F64;
+        const int bpc = enc_bytes(nd.enc);
+        const uint8_t* src = a.xyz + nd.xyz_off + (uint64_t)t.first * 3 * bpc;
+        if (staged) {
+            const uint32_t nvec = (t.count * 3u * (uint32_t)bpc + 15u) >> 4;
+            for (uint32_t v = threadIdx.x; v < nvec; v += 256) reinterpret_cast<uint4*>(sxyz)[v] = __ldcg(reinterpret_cast<const uint4*>(src) + v);
+        }
+        __syncthreads();
+        uint32_t kept_tile = 0;  // thread 0 only
+        for (uint32_t r0 = 0; r0 < t.count; r0 += 256) {
+            const uint32_t i = r0 + threadIdx.x;
+            bool keep = false;
+            if (i < t.count) {
+                double p[3];
+                if (staged) {
+                    decode_staged(sxyz, i, nd, p);
+                } else {
+#pragma unroll
+                    for (int k = 0; k < 3; ++k) p[k] = decode1_fast(load_code(src + ((size_t)i * 3 + k) * bpc, nd.enc), nd.m[k], nd.e, nd.enc);
+                }
+                keep = loc_contains(g, p[0], p[1], p[2]);
+                if (a.nfilt) {
+                    const double v = (double)a.intensity[nd.point_off + t.first + i];  // iterator.rs:82-91
+                    for (uint32_t q = 0; q < a.nfilt; ++q) keep = keep && (a.filters[q].lo <= v && v <= a.filters[q].hi);
+                }
+            }
+            const unsigned bal = __ballot_sync(0xffffffffu, keep);
+            if (lane == 0) wcnt[warp] = __popc(bal);
+            __syncthreads();
+            if (threadIdx.x == 0)
+                for (int w = 0; w < 8; ++w) kept_tile += wcnt[w];
+            __syncthreads();  // wcnt is reused by the next round
+        }
+        if (threadIdx.x == 0 && kept_tile) atomicAdd(&kept[t.loc], (unsigned long long)kept_tile);
         __syncthreads();  // sxyz is reused by the next tile
     }
 }
