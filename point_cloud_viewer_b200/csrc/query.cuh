@@ -1085,7 +1085,9 @@ __global__ void __launch_bounds__(256) k_xray_resolve(const uint32_t* __restrict
 //   1 point colour mean, 2 intensity mean (log-brightened), 3 height standard deviation through a colormap.
 // The reference accumulates per column in arrival order (f32 sums, Welford in f64) and its batches arrive from several
 // threads in unspecified order; here the columns are accumulated with atomics (f32 sums like the reference; for the
-// variance, f64 sums of (z - z0) and (z - z0)^2 around the tile's mid height), so results agree up to rounding.
+// variance, f64 sums of d = z - pivot and d^2 around a per-column pivot, the z of whichever point claims the column
+// first), so results agree up to rounding.  A pivot inside the column keeps E[d^2] - E[d]^2 free of cancellation: around
+// the tile's mid height, a 1 cm spread 1e6 m away lost every digit of its variance.
 // ------------------------------------------------------------------------------------------------
 struct XrayAttrArgs {
     XrayArgs x;
@@ -1093,9 +1095,19 @@ struct XrayAttrArgs {
     const float* intensity;  // node-contiguous intensities (mode 2)
     float* sum;              // mode 1: npix * 4; mode 2: npix
     double* dsum;            // mode 3: npix * 2
+    unsigned long long* pivot;  // mode 3: npix, the bits of the column's pivot z; kPivotEmpty until a point claims it
     uint32_t* count;
-    double z0;
 };
+constexpr unsigned long long kPivotEmpty = 0x7FF8DEADBEEF0000ull;  // a NaN payload no decoded coordinate carries
+// The column's pivot: the z of the first point to claim it with one CAS; every later point reads it.
+__device__ __forceinline__ double xray_pivot(unsigned long long* slot, double z) {
+    unsigned long long cur = *(volatile unsigned long long*)slot;
+    if (cur == kPivotEmpty) {
+        const unsigned long long prev = atomicCAS(slot, kPivotEmpty, (unsigned long long)__double_as_longlong(z));
+        cur = prev == kPivotEmpty ? (unsigned long long)__double_as_longlong(z) : prev;
+    }
+    return __longlong_as_double((long long)cur);
+}
 
 template <int MODE>
 __global__ void __launch_bounds__(256) k_xray_accum_attr(const __grid_constant__ XrayAttrArgs b) {
@@ -1132,7 +1144,7 @@ __global__ void __launch_bounds__(256) k_xray_accum_attr(const __grid_constant__
             atomicAdd(&b.sum[px], v);
             atomicAdd(&b.count[px], 1u);
         } else {
-            const double d = p[2] - b.z0;
+            const double d = p[2] - xray_pivot(&b.pivot[px], p[2]);
             atomicAdd(&b.dsum[px * 2], d);
             atomicAdd(&b.dsum[px * 2 + 1], d * d);
             atomicAdd(&b.count[px], 1u);
