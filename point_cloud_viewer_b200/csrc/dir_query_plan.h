@@ -12,6 +12,7 @@
 
 #include "../../include/pcv.h"
 #include "chain.h"
+#include "disk_io.hpp"
 
 namespace pcv {
 
@@ -98,11 +99,6 @@ struct BlobPart {
     int node;
     uint64_t header_at, xyz_at, xyz_bytes, rgb_at, rgb_bytes;
 };
-inline int find_node(const std::vector<pcv_node_meta>& nodes, uint64_t hi, uint64_t lo) {  // sorted by NodeId
-    auto it = std::lower_bound(nodes.begin(), nodes.end(), std::make_pair(hi, lo),
-                               [](const pcv_node_meta& m, const std::pair<uint64_t, uint64_t>& k) { return m.id_high != k.first ? m.id_high < k.first : m.id_low < k.second; });
-    return it != nodes.end() && it->id_high == hi && it->id_low == lo ? (int)(it - nodes.begin()) : -1;
-}
 // Per requested node, in request order: a 40-byte header, the node's position bytes, padding, its colour bytes, padding (every
 // part padded with zeros to a multiple of 8).  Returns -1, or the first request whose node is unknown or has no points (no files).
 inline int64_t nodes_blob_layout(const std::vector<pcv_node_meta>& nodes, const uint64_t* ids_hi_lo, uint32_t num, std::vector<BlobPart>& parts, uint64_t& size) {

@@ -4,15 +4,24 @@
 // Files of nodes with zero points are not created (node_writer.rs:78-89); such nodes still appear in
 // meta.pb (generation.rs:241-243).
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/pcv.h"
 
 namespace pcv {
+
+// Index of NodeId (hi, lo) in `nodes` (sorted by NodeId), -1 if absent.
+inline int find_node(const std::vector<pcv_node_meta>& nodes, uint64_t hi, uint64_t lo) {
+    auto it = std::lower_bound(nodes.begin(), nodes.end(), std::make_pair(hi, lo),
+                               [](const pcv_node_meta& m, const std::pair<uint64_t, uint64_t>& k) { return m.id_high != k.first ? m.id_high < k.first : m.id_low < k.second; });
+    return it != nodes.end() && it->id_high == hi && it->id_low == lo ? (int)(it - nodes.begin()) : -1;
+}
 
 // NodeId Display (node.rs:73-86): 'r' followed by the octal path, one digit per level.
 inline std::string node_name(uint64_t hi, uint64_t lo) {

@@ -10,6 +10,7 @@
 #include <vector>
 
 #include "../../include/pcv.h"
+#include "disk_io.hpp"
 #include "kernels_build.cuh"
 
 struct pcv_ctx {
@@ -47,20 +48,8 @@ struct pcv_octree {
     // query-side device tables, built lazily (query.cuh)
     void* d_qnodes = nullptr;
     int32_t* d_children = nullptr;     // [nodes][8] index of the child in the node table, -1 if absent
-    std::vector<int32_t> parent_of;    // index of the parent in `nodes`, -1 for the root
     std::vector<int32_t> children_of;  // 8 per node, -1 if absent
     bool tables_ready = false;
 
-    int find(uint64_t hi, uint64_t lo) const {  // `nodes` is sorted by NodeId (high, low): binary search, no side table
-        size_t a = 0, b = nodes.size();
-        while (a < b) {
-            const size_t mid = (a + b) >> 1;
-            const pcv_node_meta& m = nodes[mid];
-            if (m.id_high < hi || (m.id_high == hi && m.id_low < lo))
-                a = mid + 1;
-            else
-                b = mid;
-        }
-        return a < nodes.size() && nodes[a].id_high == hi && nodes[a].id_low == lo ? (int)a : -1;
-    }
+    int find(uint64_t hi, uint64_t lo) const { return pcv::find_node(nodes, hi, lo); }
 };

@@ -553,70 +553,7 @@ int pcv_octree_write_dir(const pcv_octree* o, const char* dir) {
     API_CATCH
 }
 
-int pcv_octree_load_dir(pcv_ctx* c, const char* dir, pcv_octree** out) {
-    if (!c || !dir || !out) return fail(PCV_ERR_INVALID, "null argument");
-    *out = nullptr;
-    API_TRY
-    const std::string d(dir);
-    std::string buf;
-    if (!read_whole_file(d + "/meta.pb", buf)) return fail(PCV_ERR_IO, "cannot read %s/meta.pb", dir);
-    MetaHeader h;
-    std::vector<ParsedNode> pn;
-    int version = 0;
-    if (!decode_meta(buf, h, pn, version))
-        return fail(PCV_ERR_INVALID, "meta.pb: unsupported or malformed (version %d; only 13 is read)", version);
-    pcv_octree* o = new pcv_octree();
-    o->ctx = c;
-    o->resolution = h.resolution;
-    uint64_t poff = 0, boff = 0;
-    if (!octree_nodes_from_meta(h, std::move(pn), o->bbox_min, o->bbox_max, o->nodes, poff, boff)) {
-        delete o;
-        return fail(PCV_ERR_INVALID, "Proto: PositionEncoding is invalid");
-    }
-    o->n = poff;
-    o->xyz_bytes = boff;
-    std::vector<uint8_t> xyz(boff), rgb(poff * 3);
-    std::vector<float> inten;
-    std::vector<uint32_t> src(poff, 0);
-    for (const auto& m : o->nodes) {
-        if (m.num_points == 0) continue;
-        const std::string stem = d + "/" + node_name(m.id_high, m.id_low);
-        const uint64_t n = (uint64_t)m.num_points, bpc = (uint64_t)enc_bytes(m.position_encoding);
-        std::string f;
-        if (!read_whole_file(stem + ".xyz", f) || f.size() != n * 3 * bpc) {
-            delete o;
-            return fail(PCV_ERR_NOT_FOUND, "node file %s.xyz missing or of wrong size", stem.c_str());
-        }
-        memcpy(xyz.data() + m.xyz_byte_offset, f.data(), f.size());
-        if (!read_whole_file(stem + ".rgb", f) || f.size() != n * 3) {
-            delete o;
-            return fail(PCV_ERR_NOT_FOUND, "node file %s.rgb missing or of wrong size", stem.c_str());
-        }
-        memcpy(rgb.data() + 3 * m.point_offset, f.data(), f.size());
-        if (read_whole_file(stem + ".intensity", f) && f.size() == n * 4) {
-            if (inten.empty()) inten.assign(poff, 0.f);
-            memcpy(inten.data() + m.point_offset, f.data(), f.size());
-        }
-    }
-    o->has_intensity = !inten.empty();
-    {
-        std::lock_guard<std::mutex> g(c->mu);
-        CU(cudaSetDevice(c->device));
-        o->d_xyz = (uint8_t*)c->be->dmalloc(boff + 32);  // + slack: the query kernels stage whole 16-byte granules
-        o->d_rgb = (uint8_t*)c->be->dmalloc(std::max<uint64_t>(poff * 3, 16));
-        o->d_src = (uint32_t*)c->be->dmalloc(std::max<uint64_t>(poff * 4, 16));
-        if (boff) c->be->h2d(o->d_xyz, xyz.data(), boff);
-        if (poff) c->be->h2d(o->d_rgb, rgb.data(), poff * 3);
-        if (poff) c->be->h2d(o->d_src, src.data(), poff * 4);
-        if (o->has_intensity) {
-            o->d_intensity = (float*)c->be->dmalloc(poff * 4);
-            c->be->h2d(o->d_intensity, inten.data(), poff * 4);
-        }
-    }
-    *out = o;
-    return PCV_OK;
-    API_CATCH
-}
+// pcv_octree_load_dir: dir_octree.inl
 
 // ---- synthetic inputs ---------------------------------------------------------------------------
 int pcv_synth_points_device(pcv_ctx* c, int kind, uint64_t seed, uint64_t first, uint64_t n, double* x, double* y, double* z, uint8_t* rgb) {

@@ -1,6 +1,7 @@
 // xray_dir_plan.h — host-only planning of the X-ray quadtree built straight from an on-disk octree (xray_dir.inl; no CUDA:
 // the CPU tests compile it with g++).
 //   octree_nodes_from_meta: meta.pb's nodes -> the node table pcv_octree_load_dir builds (no node file is read)
+//   layout_nodes:           the point and position offsets of a node table (or a subset of it) in load_dir's layout
 //   octree_children:        the 8 children of every node in that table
 //   xray_window:            the nodes a block of leaves can meet: descend from the octree root while the SAT test is not Out
 //   xray_window_size:       what one window takes in device memory (arrays, query tables, the attribute pass flags)
@@ -21,8 +22,22 @@
 
 namespace pcv {
 
+// pcv_octree_load_dir's layout of `nodes`, in table order: points node-contiguous, every node's positions 16-byte aligned.
+inline void layout_nodes(std::vector<pcv_node_meta>& nodes, uint64_t& npoints, uint64_t& xyz_bytes) {
+    uint64_t poff = 0, boff = 0;
+    for (pcv_node_meta& m : nodes) {
+        boff = (boff + 15) & ~15ull;
+        m.point_offset = poff;
+        m.xyz_byte_offset = boff;
+        poff += (uint64_t)m.num_points;
+        boff += (uint64_t)m.num_points * 3 * (uint64_t)enc_bytes(m.position_encoding);
+    }
+    npoints = poff;
+    xyz_bytes = boff;
+}
+
 // The node table of an octree directory as pcv_octree_load_dir lays it out: sorted by NodeId, cubes from the bounding cube
-// (node.rs:157-172), points node-contiguous, every node's positions 16-byte aligned.  False: an invalid position encoding.
+// (node.rs:157-172), layout_nodes' offsets.  False: an invalid position encoding.
 inline bool octree_nodes_from_meta(const MetaHeader& h, std::vector<ParsedNode> pn, double bmin[3], double bmax[3], std::vector<pcv_node_meta>& nodes,
                                    uint64_t& npoints, uint64_t& xyz_bytes) {
     typedef unsigned __int128 id128;
@@ -32,7 +47,6 @@ inline bool octree_nodes_from_meta(const MetaHeader& h, std::vector<ParsedNode> 
         bmax[a] = std::fmax(h.bbox_min[a], h.bbox_max[a]);
     }
     const double E = std::fmax(std::fmax(bmax[0] - bmin[0], bmax[1] - bmin[1]), bmax[2] - bmin[2]);
-    uint64_t poff = 0, boff = 0;
     nodes.clear();
     nodes.reserve(pn.size());
     for (const auto& p : pn) {
@@ -54,15 +68,9 @@ inline bool octree_nodes_from_meta(const MetaHeader& h, std::vector<ParsedNode> 
         }
         for (int a = 0; a < 3; ++a) m.cube_min[a] = mn[a];
         m.cube_edge = e;
-        boff = (boff + 15) & ~15ull;
-        m.point_offset = poff;
-        m.xyz_byte_offset = boff;
-        poff += (uint64_t)p.num_points;
-        boff += (uint64_t)p.num_points * 3 * (uint64_t)enc_bytes(p.enc);
         nodes.push_back(m);
     }
-    npoints = poff;
-    xyz_bytes = boff;
+    layout_nodes(nodes, npoints, xyz_bytes);
     return true;
 }
 
@@ -70,17 +78,12 @@ inline bool octree_nodes_from_meta(const MetaHeader& h, std::vector<ParsedNode> 
 inline std::vector<int32_t> octree_children(const std::vector<pcv_node_meta>& nodes) {
     typedef unsigned __int128 id128;
     std::vector<int32_t> ch(nodes.size() * 8, -1);
-    auto find = [&](uint64_t hi, uint64_t lo) -> int64_t {
-        auto it = std::lower_bound(nodes.begin(), nodes.end(), std::make_pair(hi, lo),
-                                   [](const pcv_node_meta& m, const std::pair<uint64_t, uint64_t>& k) { return m.id_high != k.first ? m.id_high < k.first : m.id_low < k.second; });
-        return it != nodes.end() && it->id_high == hi && it->id_low == lo ? (int64_t)(it - nodes.begin()) : -1;
-    };
     for (size_t i = 0; i < nodes.size(); ++i) {
         if (nodes[i].level == 0) continue;
         const id128 id = ((id128)nodes[i].id_high << 64) | nodes[i].id_low;
         const id128 idx = id & ((((id128)1) << 120) - 1);
         const id128 pid = ((id128)(nodes[i].level - 1) << 120) | (idx >> 3);  // node.rs:136-144
-        const int64_t p = find((uint64_t)(pid >> 64), (uint64_t)pid);
+        const int p = find_node(nodes, (uint64_t)(pid >> 64), (uint64_t)pid);
         if (p >= 0) ch[(size_t)p * 8 + (size_t)(idx & 7)] = (int32_t)i;
     }
     return ch;
