@@ -27,7 +27,7 @@ namespace pcv {
 #define PCV_CUDA_CHECK(x)                                                                            \
     do {                                                                                             \
         cudaError_t e_ = (x);                                                                        \
-        if (e_ != cudaSuccess) throw BuildError(-2, std::string("CUDA: ") + cudaGetErrorString(e_) + " at " #x); \
+        if (e_ != cudaSuccess) throw ::pcv::BuildError(-2, std::string("CUDA: ") + cudaGetErrorString(e_) + " at " #x); \
     } while (0)
 
 // ------------------------------------------------------------------------------------------------

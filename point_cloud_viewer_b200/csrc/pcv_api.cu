@@ -48,12 +48,6 @@ static int fail(int code, const char* fmt, ...) {
     catch (const std::bad_alloc&) { return fail(PCV_ERR_INVALID, "host out of memory"); } \
     catch (const std::exception& e) { return fail(PCV_ERR_INVALID, "%s", e.what()); }
 
-#define CU(x)                                                                                   \
-    do {                                                                                        \
-        cudaError_t e_ = (x);                                                                   \
-        if (e_ != cudaSuccess) throw BuildError(PCV_ERR_CUDA, std::string("CUDA: ") + cudaGetErrorString(e_) + " at " #x); \
-    } while (0)
-
 static void sharded_forget(pcv_ctx* c);  // sharded_build.inl: drops the slab a context still caches (no collective)
 
 extern "C" {
@@ -109,8 +103,6 @@ void pcv_destroy(pcv_ctx* c) {
     c->be->dfree(c->shard_cells);
     cudaStreamSynchronize(c->stream);
     delete c->be;
-    for (auto& p : c->ply_pin)
-        if (p) cudaFreeHost(p);
     cudaStreamDestroy(c->stream);
     delete c;
 }
@@ -127,16 +119,15 @@ static PointsView view_of(const pcv_points* p) {
     return v;
 }
 
-// Host points -> freshly allocated device copies (freed by the caller through `owned`).
-static PointsView stage_points(pcv_ctx* c, const pcv_points* hp, std::vector<void*>& owned) {
+// Host points -> freshly allocated device copies, held by `owned`.
+static PointsView stage_points(pcv_ctx* c, const pcv_points* hp, Scratch& owned) {
     PointsView v{};
     v.n = hp->n;
     const uint64_t n = hp->n;
     const uint64_t stride = hp->stride ? hp->stride : 1;
     if (n == 0) return v;
     if (stride == 3 && hp->y == hp->x + 1 && hp->z == hp->x + 2) {
-        double* d = (double*)c->be->dmalloc(n * 24);
-        owned.push_back(d);
+        double* d = owned.alloc<double>(n * 3);
         CU(cudaMemcpyAsync(d, hp->x, n * 24, cudaMemcpyHostToDevice, c->stream));
         v.x = d;
         v.y = d + 1;
@@ -149,8 +140,7 @@ static PointsView stage_points(pcv_ctx* c, const pcv_points* hp, std::vector<voi
         const double* src[3] = {hp->x, hp->y, hp->z};
         const double* dst[3];
         for (int k = 0; k < 3; ++k) {
-            double* d = (double*)c->be->dmalloc(n * 8);
-            owned.push_back(d);
+            double* d = owned.alloc<double>(n);
             CU(cudaMemcpyAsync(d, src[k], n * 8, cudaMemcpyHostToDevice, c->stream));
             dst[k] = d;
         }
@@ -162,14 +152,12 @@ static PointsView stage_points(pcv_ctx* c, const pcv_points* hp, std::vector<voi
         throw BuildError(PCV_ERR_INVALID, "positions must be SoA (stride 1) or interleaved xyz (stride 3, y=x+1, z=x+2)");
     }
     if (hp->rgb) {
-        uint8_t* r = (uint8_t*)c->be->dmalloc(n * 3);
-        owned.push_back(r);
+        uint8_t* r = owned.alloc<uint8_t>(n * 3);
         CU(cudaMemcpyAsync(r, hp->rgb, n * 3, cudaMemcpyHostToDevice, c->stream));
         v.rgb = r;
     }
     if (hp->intensity) {
-        float* f = (float*)c->be->dmalloc(n * 4);
-        owned.push_back(f);
+        float* f = owned.alloc<float>(n);
         CU(cudaMemcpyAsync(f, hp->intensity, n * 4, cudaMemcpyHostToDevice, c->stream));
         v.intensity = f;
     }
@@ -191,13 +179,12 @@ int pcv_bbox(pcv_ctx* c, const pcv_points* hp, double out_min[3], double out_max
     API_TRY
     std::lock_guard<std::mutex> g(c->mu);
     CU(cudaSetDevice(c->device));
-    std::vector<void*> owned;
+    Scratch owned(c);
     pcv_points tmp = *hp;
     tmp.rgb = nullptr;
     tmp.intensity = nullptr;
     PointsView v = stage_points(c, &tmp, owned);
     c->be->bbox(v, out_min, out_max);
-    for (void* p : owned) c->be->dfree(p);
     return PCV_OK;
     API_CATCH
 }
@@ -249,15 +236,13 @@ static int build_impl(pcv_ctx* c, const PointsView& v, double resolution, const 
     if (v.n && !v.rgb) throw BuildError(PCV_ERR_INVALID, "color is mandatory (point counts come from .rgb, on_disk.rs:23-33)");
     CudaBackend& be = *c->be;
     const uint64_t l0 = be.launches;
-    cudaEvent_t e0, e1;
-    CU(cudaEventCreate(&e0));
-    CU(cudaEventCreate(&e1));
-    CU(cudaEventRecord(e0, c->stream));
+    Events<2> ev;
+    CU(cudaEventRecord(ev.e[0], c->stream));
     BuildPlan plan(be, c->cfg.max_points_per_node, (int)c->cfg.levels_per_pass);
     if (shard) plan.shard = *shard;
     if (ext) plan.ext = *ext;
     BuildResult R = plan.run(v, resolution, bmin, bmax);
-    CU(cudaEventRecord(e1, c->stream));
+    CU(cudaEventRecord(ev.e[1], c->stream));
     CU(cudaStreamSynchronize(c->stream));
     pcv_build_stats& s = c->stats;
     s = pcv_build_stats{};
@@ -268,13 +253,11 @@ static int build_impl(pcv_ctx* c, const PointsView& v, double resolution, const 
     s.algorithmic_bytes = R.algorithmic_bytes;
     s.ms_host_plan = (float)R.host_ms_plan;
     s.ms_host_wait = (float)R.host_ms_wait;
-    cudaEventElapsedTime(&s.ms_total, e0, e1);
+    cudaEventElapsedTime(&s.ms_total, ev.e[0], ev.e[1]);
     if (v.n) {
         cudaEventElapsedTime(&s.ms_partition, be.ev[0], be.ev[1]);
         cudaEventElapsedTime(&s.ms_place, be.ev[1], be.ev[2]);
     }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
     *out = octree_from_result(c, R, resolution, bmin, bmax, v.intensity != nullptr);
     return PCV_OK;
 }
@@ -297,7 +280,7 @@ int pcv_build_octree(pcv_ctx* c, const pcv_points* hp, double resolution, const 
     API_TRY
     std::lock_guard<std::mutex> g(c->mu);
     CU(cudaSetDevice(c->device));
-    std::vector<void*> owned;
+    Scratch owned(c);
     const bool timing = std::getenv("PCV_TIMING") != nullptr;
     const auto t0 = std::chrono::steady_clock::now();
     PointsView v = stage_points(c, hp, owned);
@@ -306,15 +289,7 @@ int pcv_build_octree(pcv_ctx* c, const pcv_points* hp, double resolution, const 
         const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
         fprintf(stderr, "[pcv_build_octree] staged %.2f GB host->device in %.1f ms (%.1f GB/s)\n", hp->n * 27e-9, ms, hp->n * 27e-6 / ms);
     }
-    int rc;
-    try {
-        rc = build_impl(c, v, resolution, bbox_min, bbox_max, out);
-    } catch (...) {
-        for (void* p : owned) c->be->dfree(p);
-        throw;
-    }
-    for (void* p : owned) c->be->dfree(p);
-    return rc;
+    return build_impl(c, v, resolution, bbox_min, bbox_max, out);
     API_CATCH
 }
 
@@ -322,14 +297,8 @@ void pcv_octree_free(pcv_octree* o) {
     if (!o) return;
     pcv_ctx* c = o->ctx;
     cudaSetDevice(c->device);
-    c->be->dfree(o->d_xyz);
-    c->be->dfree(o->d_rgb);
-    c->be->dfree(o->d_intensity);
-    c->be->dfree(o->d_src);
-    c->be->dfree(o->d_qnodes);
-    c->be->dfree(o->d_children);
-    cudaStreamSynchronize(c->stream);
     delete o;
+    cudaStreamSynchronize(c->stream);
 }
 
 int pcv_device_alloc(pcv_ctx* c, uint64_t bytes, void** out) {
