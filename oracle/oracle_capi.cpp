@@ -248,6 +248,11 @@ int orc_cached_intersect_aabb(const orc_location* l, const double* mn, const dou
     return (int)isec.isec.intersect(c, 8);
 }
 int orc_location_contains(const orc_location* l, const double* p) { return to_loc(l).contains({p[0], p[1], p[2]}) ? 1 : 0; }
+// orc_location_contains of n points (xyz: n x 3, AoS) into out[n]
+void orc_location_contains_n(const orc_location* l, const double* xyz, uint64_t n, uint8_t* out) {
+    const Location loc = to_loc(l);
+    for (uint64_t i = 0; i < n; ++i) out[i] = loc.contains({xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2]}) ? 1 : 0;
+}
 void orc_location_corners(const orc_location* l, double* out24) {
     Intersector a = loc_intersector(to_loc(l));
     for (int i = 0; i < 8; ++i) {

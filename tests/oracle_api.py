@@ -84,6 +84,7 @@ def lib():
         L.orc_cached_axes.argtypes = [LP, dp, C.c_int]
         L.orc_cached_intersect_aabb.argtypes = [LP, dp, dp]
         L.orc_location_contains.argtypes = [LP, dp]
+        L.orc_location_contains_n.argtypes = [LP, C.c_void_p, C.c_uint64, C.c_void_p]
         L.orc_location_contains_sat.argtypes = [LP, dp]
         L.orc_location_corners.argtypes = [LP, dp]
         L.orc_try_inverse.argtypes = [dp, dp]
@@ -373,6 +374,14 @@ def load_dir(d):
     if not h:
         raise IOError("oracle could not load " + d)
     return OracleOctree(h)
+
+
+def location_contains(loc, xyz):
+    """Location::contains of every row of xyz (n, 3) as a bool array."""
+    xyz = np.ascontiguousarray(xyz, np.float64).reshape(-1, 3)
+    out = np.zeros(len(xyz), np.uint8)
+    lib().orc_location_contains_n(C.byref(loc), _ptr(xyz), len(xyz), _ptr(out))
+    return out.astype(bool)
 
 
 def bbox(x, y, z, stride=1):
