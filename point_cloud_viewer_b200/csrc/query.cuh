@@ -3,9 +3,10 @@
 //   k_sat_nodes      a11-a12  batched separating-axis test: (location, node cube) -> Relation
 //   k_propagate      a11      BFS semantics of NodeIdsIterator: a node is visited iff all ancestors passed
 //   k_visible_eval   a17      per node: Relation vs the view frustum + relative_size_on_screen
-//   k_cull_count / k_cull_write   a13-a15  decode + PointCulling::contains + interval filters +
-//                                 order-preserving compaction (FilteredIterator, iterator.rs:96-119)
-//   k_xray_accum / k_xray_resolve a19  discretise + per-pixel 1024-bit z-bucket set + grey mapping
+//   k_cull<0/1>, k_cull_chunk<0/1>  a13-a15  decode + PointCulling::contains + interval filters + order-preserving
+//                                   count / write passes (FilteredIterator, iterator.rs:96-119)
+//   k_cull_fused<0/1>               a13-a15  the same test in one pass: batched counts, with (1) or without (0) the survivors
+//   k_xray_bin<0/1>, k_xray_subtile a19  discretise + per-pixel 1024-bit z-bucket set + grey mapping
 //
 // All arithmetic is binary64 in the reference's operation order (compiled with -fmad=false).
 #pragma once
@@ -234,17 +235,26 @@ __device__ __forceinline__ uint64_t load_code(const uint8_t* p, int enc) {
     return *reinterpret_cast<const uint64_t*>(p);
 }
 
-__device__ __forceinline__ bool eval_point(const CullArgs& a, const QueryGeom& g, const QNode& nd, uint32_t i, double p[3]) {
-    const int bpc = enc_bytes(nd.enc);
-    const uint8_t* s = a.xyz + nd.xyz_off + (uint64_t)i * 3 * bpc;
+// Point i of node nd from the node-contiguous position codes at xyz; bpc = enc_bytes(nd.enc), computed once per node by the caller.
+__device__ __forceinline__ void decode_point(const uint8_t* xyz, const QNode& nd, int bpc, uint32_t i, double p[3]) {
+    const uint8_t* s = xyz + nd.xyz_off + (uint64_t)i * 3 * bpc;
 #pragma unroll
     for (int k = 0; k < 3; ++k) p[k] = decode1_fast(load_code(s + k * bpc, nd.enc), nd.m[k], nd.e, nd.enc);  // == decode1, integer-built unit fraction
+}
+
+// PointCulling::contains, then the interval filters on the intensity of the point at `slot`.
+__device__ __forceinline__ bool point_passes(const CullArgs& a, const QueryGeom& g, const double p[3], uint64_t slot) {
     bool keep = loc_contains(g, p[0], p[1], p[2]);
     if (a.nfilt) {
-        const double v = (double)a.intensity[nd.point_off + i];  // iterator.rs:82-91: attribute as f64, closed interval
+        const double v = (double)a.intensity[slot];  // iterator.rs:82-91: attribute as f64, closed interval
         for (uint32_t f = 0; f < a.nfilt; ++f) keep = keep && (a.filters[f].lo <= v && v <= a.filters[f].hi);
     }
     return keep;
+}
+
+__device__ __forceinline__ bool eval_point(const CullArgs& a, const QueryGeom& g, const QNode& nd, uint32_t i, double p[3]) {
+    decode_point(a.xyz, nd, enc_bytes(nd.enc), i, p);
+    return point_passes(a, g, p, nd.point_off + i);
 }
 
 // The ordered cull of one tile per block: count pass (WRITE = false), then after k_scan_u32 the write pass.  SLOT = false: the
@@ -513,6 +523,8 @@ __global__ void __launch_bounds__(256) k_pairs_to_tiles(const uint2* __restrict_
 // 256 points the block counts its survivors with ballots, reserves their output range with one atomic, stages them in shared
 // memory and copies them out as contiguous words (the order inside a round is kept; rounds land in the order they finish -
 // the batched form only promises per-location totals and the compacted set).  Survivors beyond `cap` are counted, not stored.
+// STORE = false only counts: the survivors of every tile are added to kept[loc] and nothing is stored (`cursor`, `cap` and the
+// outputs are unused), which is how a chunk of a directory-backed batched query is culled (dir_query.inl).
 struct CullFusedArgs {
     CullArgs c;
     unsigned long long* cursor;  // output slots handed out so far
@@ -535,6 +547,7 @@ __device__ __forceinline__ void decode_staged(const uint8_t* s, uint32_t i, cons
         for (int k = 0; k < 3; ++k) p[k] = decode_axis<ENC_F32>(q[k], nd.m[k], nd.e);
     }
 }
+template <bool STORE>
 __global__ void __launch_bounds__(256) k_cull_fused(const __grid_constant__ CullFusedArgs f, uint32_t ntiles) {
     __shared__ __align__(16) uint8_t sxyz[kCullStage];
     // survivors of one round of 256 points, staged so that the copy-out is contiguous 8 / 4 / 1-byte-per-lane stores
@@ -566,19 +579,21 @@ __global__ void __launch_bounds__(256) k_cull_fused(const __grid_constant__ Cull
             if (i < t.count) {
                 if (staged) {
                     decode_staged(sxyz, i, nd, p);
-                } else {
+                } else {  // Float64, from global memory: decode_point's addressing would cost this kernel 4 registers
 #pragma unroll
                     for (int k = 0; k < 3; ++k) p[k] = decode1_fast(load_code(src + ((size_t)i * 3 + k) * bpc, nd.enc), nd.m[k], nd.e, nd.enc);
                 }
-                keep = loc_contains(g, p[0], p[1], p[2]);
-                if (a.nfilt) {
-                    const double v = (double)a.intensity[nd.point_off + t.first + i];  // iterator.rs:82-91
-                    for (uint32_t q = 0; q < a.nfilt; ++q) keep = keep && (a.filters[q].lo <= v && v <= a.filters[q].hi);
-                }
+                keep = point_passes(a, g, p, nd.point_off + t.first + i);
             }
             const unsigned bal = __ballot_sync(0xffffffffu, keep);
             if (lane == 0) wcnt[warp] = __popc(bal);
             __syncthreads();
+            if (!STORE) {
+                if (threadIdx.x == 0)
+                    for (int w = 0; w < 8; ++w) kept_tile += wcnt[w];
+                __syncthreads();  // wcnt is reused by the next round
+                continue;
+            }
             uint32_t before = 0, total = 0;
 #pragma unroll
             for (int w = 0; w < 8; ++w) {
@@ -622,55 +637,6 @@ __global__ void __launch_bounds__(256) k_cull_fused(const __grid_constant__ Cull
     }
 }
 
-// The per-location count of k_cull_fused over one chunk of a directory-backed batched query: the work list holds one tile per
-// kQueryTile points of every (location, piece) pair, the positions are staged as in k_cull_fused, survivors are counted with
-// ballots and added to kept[loc] with one atomic per tile.  Nothing is stored.
-__global__ void __launch_bounds__(256) k_cull_count_chunk(const __grid_constant__ CullArgs a, uint32_t ntiles, unsigned long long* __restrict__ kept) {
-    __shared__ __align__(16) uint8_t sxyz[kCullStage];
-    __shared__ uint32_t wcnt[8];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (uint32_t ti = blockIdx.x; ti < ntiles; ti += gridDim.x) {
-        const QTile t = a.tiles[ti];
-        const QueryGeom& g = a.geoms[t.loc];
-        const QNode nd = a.nodes[t.node];
-        const bool staged = nd.enc != ENC_F64;
-        const int bpc = enc_bytes(nd.enc);
-        const uint8_t* src = a.xyz + nd.xyz_off + (uint64_t)t.first * 3 * bpc;
-        if (staged) {
-            const uint32_t nvec = (t.count * 3u * (uint32_t)bpc + 15u) >> 4;
-            for (uint32_t v = threadIdx.x; v < nvec; v += 256) reinterpret_cast<uint4*>(sxyz)[v] = __ldcg(reinterpret_cast<const uint4*>(src) + v);
-        }
-        __syncthreads();
-        uint32_t kept_tile = 0;  // thread 0 only
-        for (uint32_t r0 = 0; r0 < t.count; r0 += 256) {
-            const uint32_t i = r0 + threadIdx.x;
-            bool keep = false;
-            if (i < t.count) {
-                double p[3];
-                if (staged) {
-                    decode_staged(sxyz, i, nd, p);
-                } else {
-#pragma unroll
-                    for (int k = 0; k < 3; ++k) p[k] = decode1_fast(load_code(src + ((size_t)i * 3 + k) * bpc, nd.enc), nd.m[k], nd.e, nd.enc);
-                }
-                keep = loc_contains(g, p[0], p[1], p[2]);
-                if (a.nfilt) {
-                    const double v = (double)a.intensity[nd.point_off + t.first + i];  // iterator.rs:82-91
-                    for (uint32_t q = 0; q < a.nfilt; ++q) keep = keep && (a.filters[q].lo <= v && v <= a.filters[q].hi);
-                }
-            }
-            const unsigned bal = __ballot_sync(0xffffffffu, keep);
-            if (lane == 0) wcnt[warp] = __popc(bal);
-            __syncthreads();
-            if (threadIdx.x == 0)
-                for (int w = 0; w < 8; ++w) kept_tile += wcnt[w];
-            __syncthreads();  // wcnt is reused by the next round
-        }
-        if (threadIdx.x == 0 && kept_tile) atomicAdd(&kept[t.loc], (unsigned long long)kept_tile);
-        __syncthreads();  // sxyz is reused by the next tile
-    }
-}
-
 // ---- X-ray -----------------------------------------------------------------------------------------
 // Pixels no point falls into get TRANSPARENT.to_u8() = (255, 255, 255, 0) (src/color.rs:154-159, generation.rs:506-511).
 constexpr uint32_t kXrayTransparent = 0x00FFFFFFu;  // r | g << 8 | b << 16 | a << 24
@@ -688,8 +654,6 @@ struct XrayArgs {
     double query_from_global[7];
     int has_q;
     uint32_t w, h;
-    uint32_t* zbits;   // w*h*32
-    uint8_t* zover;    // w*h
     int* any;
 };
 
@@ -705,101 +669,79 @@ __device__ __forceinline__ uint32_t rust_as_u32_dev(double v) {
     return v != v ? 0u : u;
 }
 
-__global__ void __launch_bounds__(256) k_xray_accum(const __grid_constant__ XrayArgs a) {
-    const QTile t = a.tiles[blockIdx.x];
-    const QNode nd = a.nodes[t.node];
-    const int bpc = enc_bytes(nd.enc);
-    bool seen = false;
-    for (uint32_t i = threadIdx.x; i < t.count; i += blockDim.x) {
-        const uint8_t* s = a.xyz + nd.xyz_off + (uint64_t)(t.first + i) * 3 * bpc;
-        double p[3];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) p[k] = decode1_fast(load_code(s + k * bpc, nd.enc), nd.m[k], nd.e, nd.enc);  // == decode1, integer-built unit fraction
-        if (!loc_contains(a.geom, p[0], p[1], p[2])) continue;
-        seen = true;
-        if (a.has_q) {  // generation.rs:493-497
-            const V3 q = iso_apply(a.query_from_global, V3{p[0], p[1], p[2]});
-            p[0] = q.x;
-            p[1] = q.y;
-            p[2] = q.z;
-        }
-        // process_point_data, generation.rs:108-127 (`as u32` saturates, NaN -> 0)
-        const uint32_t x = rust_as_u32_dev(xray_unit(a, 0, p[0]) * (double)a.w);
-        const uint32_t y = rust_as_u32_dev((1. - xray_unit(a, 1, p[1])) * (double)a.h);
-        const uint32_t z = rust_as_u32_dev(xray_unit(a, 2, p[2]) * 1024.);
-        if (x < a.w && y < a.h) {
-            const size_t px = (size_t)y * a.w + x;
-            if (z < 1024)
-                atomicOr(&a.zbits[px * 32 + (z >> 5)], 1u << (z & 31));
-            else
-                a.zover[px] = 1;
-        }
+// The pixel of a point that passed the tile's location test: p is moved into the quadtree's frame when the tile has a
+// transform (generation.rs:493-497), then process_point_data (generation.rs:108-127) gives its column x, row y and z bucket.
+// The point is drawn iff x < w && y < h.
+__device__ __forceinline__ void xray_pixel(const XrayArgs& a, double p[3], uint32_t& x, uint32_t& y, uint32_t& z) {
+    if (a.has_q) {
+        const V3 q = iso_apply(a.query_from_global, V3{p[0], p[1], p[2]});
+        p[0] = q.x, p[1] = q.y, p[2] = q.z;
     }
-    if (__syncthreads_or(seen) && threadIdx.x == 0) atomicExch(a.any, 1);
+    x = rust_as_u32_dev(xray_unit(a, 0, p[0]) * (double)a.w);
+    y = rust_as_u32_dev((1. - xray_unit(a, 1, p[1])) * (double)a.h);
+    z = rust_as_u32_dev(xray_unit(a, 2, p[2]) * 1024.);
 }
 
-// The same accumulation with the z-bucket sets in SHARED memory (the global-memory form above needs 128 B per pixel: 2 GiB for
-// a 4096 x 4096 tile, written and read once more than it is used).  The points are first binned by 32 x 32 pixel sub-tile of
-// the image with a counting sort of 4-byte keys (k_xray_bin<0>: count, k_xray_bin<1>: place; octree nodes are spatially
-// coherent, so the lanes of a warp mostly share their sub-tile and the atomics are issued once per warp and sub-tile), then
-// one block per non-empty sub-tile ORs its keys into 1024 pixels x 1024 bits of shared memory (128 KB) and resolves them to
-// RGBA itself.  Per-point arithmetic and the pixel / bucket indices are exactly those of k_xray_accum.
+// The XRay strategy keeps a 1024-bit z-bucket set per pixel in SHARED memory (in global memory it would take 128 B per pixel:
+// 2 GiB for a 4096 x 4096 tile).  The points are first binned by 32 x 32 pixel sub-tile of the image with a counting sort of
+// 4-byte keys (k_xray_bin<0>: count, k_xray_bin<1>: place; octree nodes are spatially coherent, so the lanes of a warp mostly
+// share their sub-tile and the atomics are issued once per warp and sub-tile), then one block per non-empty sub-tile
+// (k_xray_subtile) ORs its keys into 1024 pixels x 1024 bits of shared memory (128 KB) and resolves them to RGBA itself.
 constexpr uint32_t kXraySub = 32;  // sub-tile edge in pixels
 struct XrayBinArgs {
-    XrayArgs x;               // geom, nodes, tiles, xyz, tile box, transform, w, h, any
+    XrayArgs x;               // geom, nodes, tiles, xyz, tile box, transform, w, h
     uint32_t ntiles;
     uint32_t sub_w;           // sub-tiles per row
     uint32_t* sub_count;      // [nsub] points per sub-tile; after the scan: exclusive offsets
     uint32_t* sub_cursor;     // [nsub] place pass: keys written so far
     uint32_t* keys;           // ly << 16 | lx << 11 | min(z, 1024)
 };
+// The count (PLACE = 0) or place (PLACE = 1) pass over work tile t of the image of `a`: every point drawn into the image goes
+// to bin bin0 + its sub-tile.  Returns whether one of the thread's points passed the location test.
 template <int PLACE>
-__global__ void __launch_bounds__(256) k_xray_bin(const __grid_constant__ XrayBinArgs b) {
-    const XrayArgs& a = b.x;
+__device__ __forceinline__ bool xray_bin_tile(const XrayArgs& a, const QNode* nodes, const uint8_t* xyz, const QTile t, uint32_t bin0, uint32_t sub_w,
+                                              uint32_t* sub_count, uint32_t* sub_cursor, uint32_t* keys) {
     const int lane = threadIdx.x & 31;
-    for (uint32_t ti = blockIdx.x; ti < b.ntiles; ti += gridDim.x) {
-        const QTile t = a.tiles[ti];
-        const QNode nd = a.nodes[t.node];
-        const int bpc = enc_bytes(nd.enc);
-        for (uint32_t i0 = 0; i0 < t.count; i0 += blockDim.x) {
-            const uint32_t i = i0 + threadIdx.x;
-            uint32_t sub = 0xFFFFFFFFu, key = 0;
-            if (i < t.count) {
-                const uint8_t* s = a.xyz + nd.xyz_off + (uint64_t)(t.first + i) * 3 * bpc;
-                double p[3];
-#pragma unroll
-                for (int k = 0; k < 3; ++k) p[k] = decode1_fast(load_code(s + k * bpc, nd.enc), nd.m[k], nd.e, nd.enc);
-                if (loc_contains(a.geom, p[0], p[1], p[2])) {
-                    if (a.has_q) {  // generation.rs:493-497
-                        const V3 q = iso_apply(a.query_from_global, V3{p[0], p[1], p[2]});
-                        p[0] = q.x, p[1] = q.y, p[2] = q.z;
-                    }
-                    // process_point_data, generation.rs:108-127 (`as u32` saturates, NaN -> 0)
-                    const uint32_t x = rust_as_u32_dev(xray_unit(a, 0, p[0]) * (double)a.w);
-                    const uint32_t y = rust_as_u32_dev((1. - xray_unit(a, 1, p[1])) * (double)a.h);
-                    const uint32_t z = rust_as_u32_dev(xray_unit(a, 2, p[2]) * 1024.);
-                    if (x < a.w && y < a.h) {
-                        sub = (y / kXraySub) * b.sub_w + (x / kXraySub);
-                        key = ((y % kXraySub) << 16) | ((x % kXraySub) << 11) | min(z, 1024u);
-                    }
-                }
-            }
-            // one atomic per warp and distinct sub-tile
-            const unsigned mask = __match_any_sync(0xffffffffu, sub);
-            if (sub != 0xFFFFFFFFu) {
-                const int leader = __ffs(mask) - 1;
-                const uint32_t rank = __popc(mask & ((1u << lane) - 1u));
-                if (PLACE) {
-                    uint32_t base = 0;
-                    if (lane == leader) base = atomicAdd(&b.sub_cursor[sub], (uint32_t)__popc(mask));
-                    base = __shfl_sync(mask, base, leader);
-                    b.keys[b.sub_count[sub] + base + rank] = key;
-                } else if (lane == leader) {
-                    atomicAdd(&b.sub_count[sub], (uint32_t)__popc(mask));
+    const QNode nd = nodes[t.node];
+    const int bpc = enc_bytes(nd.enc);
+    bool seen = false;
+    for (uint32_t i0 = 0; i0 < t.count; i0 += blockDim.x) {
+        const uint32_t i = i0 + threadIdx.x;
+        uint32_t bin = 0xFFFFFFFFu, key = 0;
+        if (i < t.count) {
+            double p[3];
+            decode_point(xyz, nd, bpc, t.first + i, p);
+            if (loc_contains(a.geom, p[0], p[1], p[2])) {
+                seen = true;
+                uint32_t x, y, z;
+                xray_pixel(a, p, x, y, z);
+                if (x < a.w && y < a.h) {
+                    bin = bin0 + (y / kXraySub) * sub_w + (x / kXraySub);
+                    key = ((y % kXraySub) << 16) | ((x % kXraySub) << 11) | min(z, 1024u);
                 }
             }
         }
+        // one atomic per warp and distinct bin
+        const unsigned mask = __match_any_sync(0xffffffffu, bin);
+        if (bin != 0xFFFFFFFFu) {
+            const int leader = __ffs(mask) - 1;
+            const uint32_t rank = __popc(mask & ((1u << lane) - 1u));
+            if (PLACE) {
+                uint32_t base = 0;
+                if (lane == leader) base = atomicAdd(&sub_cursor[bin], (uint32_t)__popc(mask));
+                base = __shfl_sync(mask, base, leader);
+                keys[sub_count[bin] + base + rank] = key;
+            } else if (lane == leader) {
+                atomicAdd(&sub_count[bin], (uint32_t)__popc(mask));
+            }
+        }
     }
+    return seen;
+}
+template <int PLACE>
+__global__ void __launch_bounds__(256) k_xray_bin(const __grid_constant__ XrayBinArgs b) {
+    for (uint32_t ti = blockIdx.x; ti < b.ntiles; ti += gridDim.x)
+        xray_bin_tile<PLACE>(b.x, b.x.nodes, b.x.xyz, b.x.tiles[ti], 0, b.sub_w, b.sub_count, b.sub_cursor, b.keys);
 }
 // The same binning for a batch of leaf tiles of one quadtree (the bounded quadtree driver, xray_api.inl): every work tile
 // carries its leaf in `loc`, every leaf has its own location and box (leaves[loc]; transform, w and h are shared), and the bins
@@ -820,52 +762,9 @@ struct XrayBatchArgs {
 };
 template <int PLACE>
 __global__ void __launch_bounds__(256) k_xray_bin_batch(const __grid_constant__ XrayBatchArgs b) {
-    const int lane = threadIdx.x & 31;
     for (uint32_t ti = blockIdx.x; ti < b.ntiles; ti += gridDim.x) {
         const QTile t = b.tiles[ti];
-        const XrayArgs& a = b.leaves[t.loc];
-        const QNode nd = b.nodes[t.node];
-        const int bpc = enc_bytes(nd.enc);
-        bool seen = false;
-        for (uint32_t i0 = 0; i0 < t.count; i0 += blockDim.x) {
-            const uint32_t i = i0 + threadIdx.x;
-            uint32_t bin = 0xFFFFFFFFu, key = 0;
-            if (i < t.count) {
-                const uint8_t* s = b.xyz + nd.xyz_off + (uint64_t)(t.first + i) * 3 * bpc;
-                double p[3];
-#pragma unroll
-                for (int k = 0; k < 3; ++k) p[k] = decode1_fast(load_code(s + k * bpc, nd.enc), nd.m[k], nd.e, nd.enc);
-                if (loc_contains(a.geom, p[0], p[1], p[2])) {
-                    seen = true;
-                    if (a.has_q) {  // generation.rs:493-497
-                        const V3 q = iso_apply(a.query_from_global, V3{p[0], p[1], p[2]});
-                        p[0] = q.x, p[1] = q.y, p[2] = q.z;
-                    }
-                    // process_point_data, generation.rs:108-127, exactly as in k_xray_bin
-                    const uint32_t x = rust_as_u32_dev(xray_unit(a, 0, p[0]) * (double)a.w);
-                    const uint32_t y = rust_as_u32_dev((1. - xray_unit(a, 1, p[1])) * (double)a.h);
-                    const uint32_t z = rust_as_u32_dev(xray_unit(a, 2, p[2]) * 1024.);
-                    if (x < a.w && y < a.h) {
-                        bin = t.loc * b.nsub + (y / kXraySub) * b.sub_w + (x / kXraySub);
-                        key = ((y % kXraySub) << 16) | ((x % kXraySub) << 11) | min(z, 1024u);
-                    }
-                }
-            }
-            // one atomic per warp and distinct bin
-            const unsigned mask = __match_any_sync(0xffffffffu, bin);
-            if (bin != 0xFFFFFFFFu) {
-                const int leader = __ffs(mask) - 1;
-                const uint32_t rank = __popc(mask & ((1u << lane) - 1u));
-                if (PLACE) {
-                    uint32_t base = 0;
-                    if (lane == leader) base = atomicAdd(&b.sub_cursor[bin], (uint32_t)__popc(mask));
-                    base = __shfl_sync(mask, base, leader);
-                    b.keys[b.sub_count[bin] + base + rank] = key;
-                } else if (lane == leader) {
-                    atomicAdd(&b.sub_count[bin], (uint32_t)__popc(mask));
-                }
-            }
-        }
+        const bool seen = xray_bin_tile<PLACE>(b.leaves[t.loc], b.nodes, b.xyz, t, t.loc * b.nsub, b.sub_w, b.sub_count, b.sub_cursor, b.keys);
         if (!PLACE && __syncthreads_or(seen) && threadIdx.x == 0) b.seen[t.loc] = 1;
     }
 }
@@ -920,10 +819,8 @@ __global__ void __launch_bounds__(256) k_xray_occupy(const __grid_constant__ Xra
         const QNode nd = a.nodes[t.node];
         const int bpc = enc_bytes(nd.enc);
         for (uint32_t i = threadIdx.x; i < t.count; i += blockDim.x) {
-            const uint8_t* s = a.xyz + nd.xyz_off + (uint64_t)(t.first + i) * 3 * bpc;
             double p[3];
-#pragma unroll
-            for (int k = 0; k < 3; ++k) p[k] = decode1_fast(load_code(s + k * bpc, nd.enc), nd.m[k], nd.e, nd.enc);
+            decode_point(a.xyz, nd, bpc, t.first + i, p);
             int64_t x0, x1, y0, y1;
             xray_point_cells(p, a.has_q ? a.query_from_global : nullptr, a.x0, a.y0, a.edge, a.margin, cells, x0, x1, y0, y1);
             for (int64_t ix = x0; ix <= x1; ++ix)
@@ -990,10 +887,8 @@ __global__ void __launch_bounds__(256) k_xray_occupy_cells(const __grid_constant
         const QNode nd = a.nodes[t.node];
         const int bpc = enc_bytes(nd.enc);
         for (uint32_t i = threadIdx.x; i < t.count; i += blockDim.x) {
-            const uint8_t* s = a.xyz + nd.xyz_off + (uint64_t)(t.first + i) * 3 * bpc;
             double p[3];
-#pragma unroll
-            for (int k = 0; k < 3; ++k) p[k] = decode1_fast(load_code(s + k * bpc, nd.enc), nd.m[k], nd.e, nd.enc);
+            decode_point(a.xyz, nd, bpc, t.first + i, p);
             int64_t x0, x1, y0, y1;
             xray_point_cells(p, a.has_q ? a.query_from_global : nullptr, a.x0, a.y0, a.edge, a.margin, cells, x0, x1, y0, y1);
             for (int64_t ix = x0; ix <= x1; ++ix)
@@ -1005,7 +900,6 @@ __global__ void __launch_bounds__(256) k_xray_occupy_cells(const __grid_constant
     }
 }
 struct XraySubArgs {
-    const uint32_t* sub_id;     // unused (every sub-tile has a block; empty ones leave at once)
     const uint32_t* sub_off;    // [nleaf * nsub + 1] exclusive offsets into keys
     const uint32_t* keys;
     const uint8_t* grey;        // [1026]
@@ -1060,26 +954,6 @@ __global__ void __launch_bounds__(512, 1) k_xray_subtile(const __grid_constant__
     }
 }
 
-// grey[count] LUT is computed on the host with libm log (generation.rs:186-197) so the cast boundary matches.
-__global__ void __launch_bounds__(256) k_xray_resolve(const uint32_t* __restrict__ zbits, const uint8_t* __restrict__ zover,
-                                                      const uint8_t* __restrict__ grey, uint32_t npix, uint8_t* __restrict__ rgba) {
-    const uint32_t px = blockIdx.x * blockDim.x + threadIdx.x;
-    if (px >= npix) return;
-    uint32_t cnt = zover[px];
-    const uint4* b = reinterpret_cast<const uint4*>(zbits + (size_t)px * 32);
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-        const uint4 v = b[k];
-        cnt += __popc(v.x) + __popc(v.y) + __popc(v.z) + __popc(v.w);
-    }
-    uchar4 o = make_uchar4(255, 255, 255, 0);  // TRANSPARENT.to_u8() (color.rs:154-159; generation.rs:506-511)
-    if (cnt) {
-        const uint8_t gval = grey[cnt];
-        o = make_uchar4(gval, gval, gval, 255);
-    }
-    reinterpret_cast<uchar4*>(rgba)[px] = o;
-}
-
 // ------------------------------------------------------------------------------------------------
 // The other colouring strategies of the X-ray tiles (xray/src/generation.rs:200-405), Binning = None:
 //   1 point colour mean, 2 intensity mean (log-brightened), 3 height standard deviation through a colormap.
@@ -1117,18 +991,12 @@ __global__ void __launch_bounds__(256) k_xray_accum_attr(const __grid_constant__
     const int bpc = enc_bytes(nd.enc);
     bool seen = false;
     for (uint32_t i = threadIdx.x; i < t.count; i += blockDim.x) {
-        const uint8_t* s = a.xyz + nd.xyz_off + (uint64_t)(t.first + i) * 3 * bpc;
         double p[3];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) p[k] = decode1_fast(load_code(s + k * bpc, nd.enc), nd.m[k], nd.e, nd.enc);
+        decode_point(a.xyz, nd, bpc, t.first + i, p);
         if (!loc_contains(a.geom, p[0], p[1], p[2])) continue;
         seen = true;
-        if (a.has_q) {
-            const V3 q = iso_apply(a.query_from_global, V3{p[0], p[1], p[2]});
-            p[0] = q.x, p[1] = q.y, p[2] = q.z;
-        }
-        const uint32_t x = rust_as_u32_dev(xray_unit(a, 0, p[0]) * (double)a.w);
-        const uint32_t y = rust_as_u32_dev((1. - xray_unit(a, 1, p[1])) * (double)a.h);
+        uint32_t x, y, z;
+        xray_pixel(a, p, x, y, z);
         if (!(x < a.w && y < a.h)) continue;
         const size_t px = (size_t)y * a.w + x;
         const uint64_t slot = nd.point_off + t.first + i;

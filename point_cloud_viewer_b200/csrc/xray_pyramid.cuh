@@ -54,8 +54,7 @@ struct XrayBinnedArgs {
     double bin_size;
     BinnedTables t;
 };
-// Per point: exactly the discretisation of k_xray_accum_attr (process_point_data, generation.rs:108-127), then the
-// (pixel, bin) hash aggregation of xray_pyramid.h.
+// Per point: the pixel of k_xray_accum_attr (xray_pixel), then the (pixel, bin) hash aggregation of xray_pyramid.h.
 template <int MODE>
 __global__ void __launch_bounds__(256) k_xray_binned_insert(const __grid_constant__ XrayBinnedArgs b) {
     const XrayArgs& a = b.x;
@@ -64,18 +63,12 @@ __global__ void __launch_bounds__(256) k_xray_binned_insert(const __grid_constan
     const int bpc = enc_bytes(nd.enc);
     bool seen = false;
     for (uint32_t i = threadIdx.x; i < t.count; i += blockDim.x) {
-        const uint8_t* s = a.xyz + nd.xyz_off + (uint64_t)(t.first + i) * 3 * bpc;
         double p[3];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) p[k] = decode1_fast(load_code(s + k * bpc, nd.enc), nd.m[k], nd.e, nd.enc);
+        decode_point(a.xyz, nd, bpc, t.first + i, p);
         if (!loc_contains(a.geom, p[0], p[1], p[2])) continue;
         seen = true;
-        if (a.has_q) {
-            const V3 q = iso_apply(a.query_from_global, V3{p[0], p[1], p[2]});
-            p[0] = q.x, p[1] = q.y, p[2] = q.z;
-        }
-        const uint32_t x = rust_as_u32_dev(xray_unit(a, 0, p[0]) * (double)a.w);
-        const uint32_t y = rust_as_u32_dev((1. - xray_unit(a, 1, p[1])) * (double)a.h);
+        uint32_t x, y, z;
+        xray_pixel(a, p, x, y, z);
         if (!(x < a.w && y < a.h)) continue;
         const uint32_t px = y * a.w + x;
         const uint64_t slot = nd.point_off + t.first + i;

@@ -7,9 +7,9 @@ on the special intensities (interval ends, -0.0, NaN, +-inf, an f32 subnormal, f
   k_sat_nodes        nodes_in_location (resident and OctreeDir) equals the oracle's
   k_cull             Octree.query_points streams exactly the oracle's points; the survivors are the float64 reference's
   k_bfs_level +      query_batch_device: every count is the reference's, every `tested` the oracle's
-    k_cull_fused
+    k_cull_fused<true>
   k_cull_chunk       OctreeDir.query_points equals the resident stream, at the smallest accepted budget and the default one
-  k_cull_count_chunk OctreeDir.query_batch counts are the reference's
+  k_cull_fused<false> OctreeDir.query_batch counts are the reference's
   k_lod_shuffle      shuffle_nodes equals the oracle's reshuffle for every encoding's bytes per coordinate
 """
 import numpy as np
@@ -177,7 +177,7 @@ def test_octree_dir_at_the_edges(scene):
         # nodes then still run in many chunks.
         nb = 8 if budget == small else len(plocs)
         hb = pcv.OctreeDir(ctx, s["dir"], small + nb * (4096 + 24 * h.num_nodes) + (64 << 10)) if budget == small else h
-        # k_cull_count_chunk's copy of the interval filter: every filter edge at the default budget, f32 0.1 in many chunks
+        # k_cull_fused<false>'s interval filter: every filter edge at the default budget, f32 0.1 in many chunks
         for filters in [()] + (R.FILTERS if budget != small else [R.FILTERS[3]]):
             parts, chunks = [], 0
             for i in range(0, len(plocs), nb):
