@@ -159,6 +159,24 @@ int pcv_query_points(const pcv_octree* o, const pcv_location* loc, const pcv_int
 int pcv_query_batch_device(const pcv_octree* o, const pcv_location* locs, uint32_t nloc, const pcv_interval* filters,
                            uint32_t nfilt, uint64_t* counts_out, uint64_t* tested_out);
 
+/* ---- PointLocation::S2Cells: queries by S2 cell union (src/geometry/s2_cell_union.rs) ------ */
+/* A point passes iff the union contains the leaf cell of its decoded position (CellUnion::contains(CellID::from_point(p))).
+ * The ids are validated and normalised (CellUnion::normalize); an invalid id, or n > 0 with ids == NULL, is PCV_ERR_INVALID.
+ * An empty union selects no node and returns no point.  The points equal every point of the octree that passes the test, in
+ * the order the AllPoints stream delivers them.  The node list holds every node with a passing point, in BFS order; it is not
+ * the reference's list (which pre-selects with latitude / longitude rectangles): it may hold nodes without one. */
+typedef struct pcv_cell_union {
+    const uint64_t* ids;
+    uint32_t n;
+    uint32_t pad;
+} pcv_cell_union;
+int pcv_nodes_in_cell_union(const pcv_octree* o, const pcv_cell_union* cu, uint64_t* ids_hi_lo, uint64_t cap, uint64_t* n_out);
+int pcv_query_cell_union(const pcv_octree* o, const pcv_cell_union* cu, const pcv_interval* filters, uint32_t nfilt,
+                         uint64_t batch_size, pcv_batch_cb cb, void* user);
+/* pcv_query_batch_device over nunion cell unions; fills pcv_last_query_stats the same way. */
+int pcv_query_cell_unions_batch_device(const pcv_octree* o, const pcv_cell_union* unions, uint32_t nunion, const pcv_interval* filters,
+                                       uint32_t nfilt, uint64_t* counts_out, uint64_t* tested_out);
+
 /* Timing / traffic of the last pcv_query_batch_device call on the context (CUDA events on the context's stream). */
 typedef struct pcv_query_stats {
     float ms_device;            /* first kernel to last kernel of the call                                   */
@@ -331,6 +349,12 @@ int pcv_octree_dir_query_points(const pcv_octree_dir* d, const pcv_location* loc
  * does not fit what the budget leaves -> PCV_ERR_UNSUPPORTED ("split the batch"). */
 int pcv_octree_dir_query_batch(const pcv_octree_dir* d, const pcv_location* locs, uint32_t nloc, const pcv_interval* filters,
                                uint32_t nfilt, uint64_t* counts_out, uint64_t* tested_out);
+/* The cell-union calls over the directory (src_index = slot, max_device_bytes bounds the unions' tables too). */
+int pcv_octree_dir_nodes_in_cell_union(const pcv_octree_dir* d, const pcv_cell_union* cu, uint64_t* ids_hi_lo, uint64_t cap, uint64_t* n_out);
+int pcv_octree_dir_query_cell_union(const pcv_octree_dir* d, const pcv_cell_union* cu, const pcv_interval* filters, uint32_t nfilt,
+                                    uint64_t batch_size, pcv_batch_cb cb, void* user);
+int pcv_octree_dir_query_cell_unions_batch(const pcv_octree_dir* d, const pcv_cell_union* unions, uint32_t nunion, const pcv_interval* filters,
+                                           uint32_t nfilt, uint64_t* counts_out, uint64_t* tested_out);
 /* pcv_nodes_data_blob's reply, read from the node files straight into `out` on the host. */
 int pcv_octree_dir_nodes_data_blob(const pcv_octree_dir* d, const uint64_t* ids_hi_lo, uint32_t num_nodes, void* out, uint64_t cap,
                                    uint64_t* size_out);

@@ -143,6 +143,19 @@ class Context {
     pcv_ctx* h_ = nullptr;
 };
 
+using CellID = uint64_t;                 // s2::cellid::CellID(u64)
+using CellUnion = std::vector<CellID>;   // s2::cellunion::CellUnion(Vec<CellID>)
+
+// The octree queries by cell union (PointLocation::S2Cells) shared by Octree and OctreeDir, over their pcv_* entry points.
+namespace detail {
+inline pcv_cell_union raw_union(const CellUnion& cu) { return pcv_cell_union{cu.data(), (uint32_t)cu.size(), 0}; }
+inline std::vector<pcv_cell_union> raw_unions(const std::vector<CellUnion>& us) {
+    std::vector<pcv_cell_union> raw;
+    for (auto& u : us) raw.push_back(raw_union(u));
+    return raw;
+}
+}  // namespace detail
+
 struct NodeData {  // octree/mod.rs:147-152
     pcv_node_meta meta;
     std::vector<uint8_t> position, color;
@@ -179,6 +192,25 @@ class Octree {
         uint64_t n = 0;
         check(pcv_nodes_in_location(o_, &loc.raw, ids.data(), nodes_.size(), &n));
         return to_ids(ids, n);
+    }
+    // PointLocation::S2Cells: every node that holds a point whose leaf cell the union contains, in BFS order
+    std::vector<NodeId> nodes_in_location(const CellUnion& cell_union) const {
+        std::vector<uint64_t> ids(2 * nodes_.size() + 2);
+        uint64_t n = 0;
+        const pcv_cell_union cu = detail::raw_union(cell_union);
+        check(pcv_nodes_in_cell_union(o_, &cu, ids.data(), nodes_.size(), &n));
+        return to_ids(ids, n);
+    }
+    // The points of PointLocation::S2Cells(cell_union) that pass the filter intervals, in batches of `batch_size` points (the
+    // last one short), in AllPoints order; func returns false to stop.  Returns true if every batch was consumed.
+    bool for_each_batch(const CellUnion& cell_union, const std::vector<ClosedInterval>& filter_intervals, size_t batch_size,
+                        const std::function<bool(PointsBatch&&)>& func) const;
+    // survivors and tested points of every cell union
+    void query_batch(const std::vector<CellUnion>& unions, std::vector<uint64_t>& counts, std::vector<uint64_t>& tested) const {
+        const std::vector<pcv_cell_union> raw = detail::raw_unions(unions);
+        counts.assign(unions.size(), 0);
+        tested.assign(unions.size(), 0);
+        check(pcv_query_cell_unions_batch_device(o_, raw.data(), (uint32_t)raw.size(), nullptr, 0, counts.data(), tested.data()));
     }
     NodeData get_node_data(const NodeId& id) const {  // mod.rs:285-307
         for (auto& m : nodes_)
@@ -269,6 +301,32 @@ inline PointsBatch batch_from(const pcv_batch* b) {
     return pb;
 }
 
+namespace detail {
+// One streaming call (query(cb, user)) with `func` as the consumer: false if func stopped it.
+template <class Q>
+inline bool stream_batches(const std::function<bool(PointsBatch&&)>& func, Q&& query) {
+    auto tramp = [](void* user, const pcv_batch* b) -> int { return (*(const std::function<bool(PointsBatch&&)>*)user)(batch_from(b)) ? 0 : 1; };
+    const int rc = query(+tramp, (void*)&func);
+    if (rc == PCV_ERR_CANCELLED) return false;
+    check(rc);
+    return true;
+}
+inline std::vector<pcv_interval> raw_intervals(const std::vector<ClosedInterval>& iv) {
+    std::vector<pcv_interval> f;
+    for (auto& i : iv) f.push_back(pcv_interval{i.lower_bound, i.upper_bound});
+    return f;
+}
+}  // namespace detail
+
+inline bool Octree::for_each_batch(const CellUnion& cell_union, const std::vector<ClosedInterval>& filter_intervals, size_t batch_size,
+                                   const std::function<bool(PointsBatch&&)>& func) const {
+    const pcv_cell_union cu = detail::raw_union(cell_union);
+    const std::vector<pcv_interval> f = detail::raw_intervals(filter_intervals);
+    return detail::stream_batches(func, [&](pcv_batch_cb cb, void* user) {
+        return pcv_query_cell_union(o_, &cu, f.empty() ? nullptr : f.data(), (uint32_t)f.size(), batch_size, cb, user);
+    });
+}
+
 // An octree directory queried where it lies (Octree over OnDiskDataProvider, octree/mod.rs:156-215, 337-352): the node table is
 // on the device and every query reads only the nodes it selects, within `max_device_bytes`.  Results equal Octree::from_directory's;
 // a batch's source_index is the point's slot in nodes() (point_offset + j of its node).
@@ -316,6 +374,28 @@ class OctreeDir {
         counts.assign(locs.size(), 0);
         tested.assign(locs.size(), 0);
         check(pcv_octree_dir_query_batch(d_, raw.data(), (uint32_t)raw.size(), nullptr, 0, counts.data(), tested.data()));
+    }
+    // The cell-union forms of Octree's, over the directory (source_index = slot)
+    std::vector<NodeId> nodes_in_location(const CellUnion& cell_union) const {
+        std::vector<uint64_t> ids(2 * nodes_.size() + 2);
+        uint64_t n = 0;
+        const pcv_cell_union cu = detail::raw_union(cell_union);
+        check(pcv_octree_dir_nodes_in_cell_union(d_, &cu, ids.data(), nodes_.size(), &n));
+        return to_ids(ids, n);
+    }
+    bool for_each_batch(const CellUnion& cell_union, const std::vector<ClosedInterval>& filter_intervals, size_t batch_size,
+                        const std::function<bool(PointsBatch&&)>& func) const {
+        const pcv_cell_union cu = detail::raw_union(cell_union);
+        const std::vector<pcv_interval> f = detail::raw_intervals(filter_intervals);
+        return detail::stream_batches(func, [&](pcv_batch_cb cb, void* user) {
+            return pcv_octree_dir_query_cell_union(d_, &cu, f.empty() ? nullptr : f.data(), (uint32_t)f.size(), batch_size, cb, user);
+        });
+    }
+    void query_batch(const std::vector<CellUnion>& unions, std::vector<uint64_t>& counts, std::vector<uint64_t>& tested) const {
+        const std::vector<pcv_cell_union> raw = detail::raw_unions(unions);
+        counts.assign(unions.size(), 0);
+        tested.assign(unions.size(), 0);
+        check(pcv_octree_dir_query_cell_unions_batch(d_, raw.data(), (uint32_t)raw.size(), nullptr, 0, counts.data(), tested.data()));
     }
     std::vector<uint8_t> nodes_data_blob(const std::vector<NodeId>& ids) const {
         std::vector<uint64_t> hl;
@@ -391,8 +471,6 @@ inline Octree build_octree_from_file(Context& ctx, const std::string& output_dir
 }
 
 // ---- the S2-cell point cloud: point_viewer::s2_cells::S2Cells + read_write::S2Splitter (src/s2_cells/mod.rs, src/read_write/s2.rs) ----
-using CellID = uint64_t;                 // s2::cellid::CellID(u64)
-using CellUnion = std::vector<CellID>;   // s2::cellunion::CellUnion(Vec<CellID>)
 
 // CellID::to_token (the per-cell file stem of the S2 directory layout)
 inline std::string cell_token(CellID id) {

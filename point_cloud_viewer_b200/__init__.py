@@ -566,13 +566,9 @@ class Octree:
     def write_dir(self, directory):
         N.check(N.lib().pcv_octree_write_dir(self.h, str(directory).encode()))
 
-    # PointCloud::nodes_in_location (octree/mod.rs:329-331)
+    # PointCloud::nodes_in_location (octree/mod.rs:329-331); `loc` is a pcv_location or a geometry.CellUnion
     def nodes_in_location(self, loc):
-        cap = len(self.nodes) + 1
-        out = np.zeros(2 * cap, np.uint64)
-        n = C.c_uint64()
-        N.check(N.lib().pcv_nodes_in_location(self.h, C.byref(loc), _p(out), cap, C.byref(n)))
-        return [node_name(out[2 * i], out[2 * i + 1]) for i in range(n.value)]
+        return _nodes_in(N.lib().pcv_nodes_in_location, N.lib().pcv_nodes_in_cell_union, self.h, loc, len(self.nodes) + 1)
 
     # Octree::get_visible_nodes (octree/mod.rs:228)
     def get_visible_nodes(self, clip_from_world):
@@ -587,11 +583,14 @@ class Octree:
     # ParallelIterator::try_for_each_batch semantics (iterator.rs:255-333) on the caller's thread
     def query_points(self, loc, callback=None, filters=(), batch_size=500000):
         """Streams batches dict(xyz (n,3) f64, rgb (n,3), intensity, src).  A callback returning a truthy
-        value cancels the stream (ErrorKind::Channel); without a callback the batches are returned."""
-        return _query_points(N.lib().pcv_query_points, self.h, loc, callback, filters, batch_size)
+        value cancels the stream (ErrorKind::Channel); without a callback the batches are returned.  `loc` is a pcv_location
+        or a geometry.CellUnion."""
+        fn = N.lib().pcv_query_cell_union if isinstance(loc, geometry.CellUnion) else N.lib().pcv_query_points
+        return _query_points(fn, self.h, loc, callback, filters, batch_size)
 
     def query_batch_device(self, locs, filters=()):
-        return _query_batch(N.lib().pcv_query_batch_device, self.h, locs, filters)
+        """(counts, tested) per location; the locations are all pcv_locations or all geometry.CellUnions."""
+        return _query_batch(N.lib().pcv_query_batch_device, N.lib().pcv_query_cell_unions_batch_device, self.h, locs, filters)
 
     def last_query_stats(self):
         """Timing / traffic of the last query_batch_device call (pcv_query_stats)."""
@@ -660,7 +659,21 @@ class Octree:
         return _xray_info(info, binfo)
 
 
+def _loc_arg(loc):
+    """The C argument of one location: the pcv_location itself, or the pcv_cell_union view of a geometry.CellUnion."""
+    return loc.struct() if isinstance(loc, geometry.CellUnion) else loc
+
+
+def _nodes_in(fn_loc, fn_union, h, loc, cap):
+    out = np.zeros(2 * cap, np.uint64)
+    n = C.c_uint64()
+    arg = _loc_arg(loc)
+    N.check((fn_union if isinstance(loc, geometry.CellUnion) else fn_loc)(h, C.byref(arg), _p(out), cap, C.byref(n)))
+    return [node_name(out[2 * i], out[2 * i + 1]) for i in range(n.value)]
+
+
 def _query_points(fn, h, loc, callback, filters, batch_size):
+    loc = _loc_arg(loc)
     f = np.asarray(filters, np.float64).reshape(-1)
     nf = len(f) // 2
     got = []
@@ -687,8 +700,15 @@ def _query_points(fn, h, loc, callback, filters, batch_size):
     return got
 
 
-def _query_batch(fn, h, locs, filters):
-    arr = (N.Location * len(locs))(*locs)
+def _query_batch(fn, fn_union, h, locs, filters):
+    unions = [isinstance(loc, geometry.CellUnion) for loc in locs]
+    if any(unions):
+        if not all(unions):
+            raise ValueError("a batch of locations holds cell unions and other locations; query them in separate batches")
+        arr = (N.CellUnion * len(locs))(*[loc.struct() for loc in locs])
+        fn = fn_union
+    else:
+        arr = (N.Location * len(locs))(*locs)
     f = np.asarray(filters, np.float64).reshape(-1)
     nf = len(f) // 2
     counts, tested = np.zeros(len(locs), np.uint64), np.zeros(len(locs), np.uint64)
@@ -732,11 +752,7 @@ class OctreeDir:
             pass
 
     def nodes_in_location(self, loc):
-        cap = self.num_nodes + 1
-        out = np.zeros(2 * cap, np.uint64)
-        n = C.c_uint64()
-        N.check(N.lib().pcv_octree_dir_nodes_in_location(self.h, C.byref(loc), _p(out), cap, C.byref(n)))
-        return [node_name(out[2 * i], out[2 * i + 1]) for i in range(n.value)]
+        return _nodes_in(N.lib().pcv_octree_dir_nodes_in_location, N.lib().pcv_octree_dir_nodes_in_cell_union, self.h, loc, self.num_nodes + 1)
 
     def get_visible_nodes(self, clip_from_world):
         m = np.asarray(clip_from_world, np.float64)
@@ -749,11 +765,12 @@ class OctreeDir:
 
     def query_points(self, loc, callback=None, filters=(), batch_size=500000):
         """Octree.query_points over the directory; `src` holds every point's slot."""
-        return _query_points(N.lib().pcv_octree_dir_query_points, self.h, loc, callback, filters, batch_size)
+        fn = N.lib().pcv_octree_dir_query_cell_union if isinstance(loc, geometry.CellUnion) else N.lib().pcv_octree_dir_query_points
+        return _query_points(fn, self.h, loc, callback, filters, batch_size)
 
     def query_batch(self, locs, filters=()):
         """(counts, tested) of Octree.query_batch_device, every visited node read once."""
-        return _query_batch(N.lib().pcv_octree_dir_query_batch, self.h, locs, filters)
+        return _query_batch(N.lib().pcv_octree_dir_query_batch, N.lib().pcv_octree_dir_query_cell_unions_batch, self.h, locs, filters)
 
     def nodes_data_blob(self, names, out=None):
         ids = np.zeros(2 * len(names), np.uint64)

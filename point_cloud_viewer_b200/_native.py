@@ -70,6 +70,10 @@ class Location(C.Structure):
     ]
 
 
+class CellUnion(C.Structure):  # pcv_cell_union
+    _fields_ = [("ids", C.c_void_p), ("n", C.c_uint32), ("pad", C.c_uint32)]
+
+
 class Interval(C.Structure):
     _fields_ = [("lo", C.c_double), ("hi", C.c_double)]
 
@@ -208,6 +212,9 @@ SYMBOLS = [
     ("pcv_visible_nodes", C.c_int, [C.c_void_p, _dp, C.c_void_p, C.c_uint64, _u64p]),
     ("pcv_query_points", C.c_int, [C.c_void_p, C.POINTER(Location), C.c_void_p, C.c_uint32, C.c_uint64, BATCH_CB, C.c_void_p]),
     ("pcv_query_batch_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
+    ("pcv_nodes_in_cell_union", C.c_int, [C.c_void_p, C.POINTER(CellUnion), C.c_void_p, C.c_uint64, _u64p]),
+    ("pcv_query_cell_union", C.c_int, [C.c_void_p, C.POINTER(CellUnion), C.c_void_p, C.c_uint32, C.c_uint64, BATCH_CB, C.c_void_p]),
+    ("pcv_query_cell_unions_batch_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
     ("pcv_last_query_stats", C.c_int, [C.c_void_p, C.POINTER(QueryStats)]),
     ("pcv_last_xray_stats", C.c_int, [C.c_void_p, C.POINTER(XrayStats)]),
     ("pcv_xray_tile", C.c_int, [C.c_void_p, _dp, _dp, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]),
@@ -233,6 +240,9 @@ SYMBOLS = [
     ("pcv_octree_dir_visible_nodes", C.c_int, [C.c_void_p, _dp, C.c_void_p, C.c_uint64, _u64p]),
     ("pcv_octree_dir_query_points", C.c_int, [C.c_void_p, C.POINTER(Location), C.c_void_p, C.c_uint32, C.c_uint64, BATCH_CB, C.c_void_p]),
     ("pcv_octree_dir_query_batch", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
+    ("pcv_octree_dir_nodes_in_cell_union", C.c_int, [C.c_void_p, C.POINTER(CellUnion), C.c_void_p, C.c_uint64, _u64p]),
+    ("pcv_octree_dir_query_cell_union", C.c_int, [C.c_void_p, C.POINTER(CellUnion), C.c_void_p, C.c_uint32, C.c_uint64, BATCH_CB, C.c_void_p]),
+    ("pcv_octree_dir_query_cell_unions_batch", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
     ("pcv_octree_dir_nodes_data_blob", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, _u64p]),
     ("pcv_octree_dir_last_stats", C.c_int, [C.c_void_p, C.POINTER(DirQueryStats)]),
     ("pcv_s2_cell_ids", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_uint32, C.c_void_p]),

@@ -12,6 +12,7 @@
 #include <limits>
 
 #include "../../include/pcv.h"
+#include "s2.h"
 
 namespace pcv {
 
@@ -60,16 +61,23 @@ PCV_GHD V3 iso_apply(const double* iso7, V3 p) {
     return V3{r.x + iso7[0], r.y + iso7[1], r.z + iso7[2]};
 }
 
+// The kind of a QueryGeom built from a cell union (PointLocation::S2Cells, src/iterator.rs:13-20).  Internal: pcv_location has no
+// such kind; the cell-union entry points build the geometry themselves.
+constexpr int32_t kLocCellUnion = 16;
+
 // What the device needs per location.
 struct QueryGeom {
     int32_t kind;
-    int32_t naxes;       // cached separating axes (<= 26); 0 for AllPoints
+    int32_t naxes;       // cached separating axes (<= 26); 0 for AllPoints and cell unions
     double axes[26][3];
     double corners[8][3];
     double aabb_min[3], aabb_max[3];
     double clip_from_query[16];
     double obb_from_query[7];
     double half_extent[3];
+    const uint64_t* cells;     // cell union: its normalised ids (device) ...
+    const S2Square* squares;   // ... and each one's face and square of leaf cells (device)
+    uint32_t ncells, pad;
 };
 
 inline V3 unit(V3 v) {

@@ -30,6 +30,7 @@ struct QNode {
 };
 
 enum : uint8_t { REL_IN = 0, REL_CROSS = 1, REL_OUT = 2 };  // sat.rs:39-47
+static_assert((int)REL_IN == kS2RelIn && (int)REL_CROSS == kS2RelCross && (int)REL_OUT == kS2RelOut, "s2_cube_relation returns a Relation");
 
 // Project the 8 corners of the cube (min m, edge e) on an axis: Aabb corners order x fastest (aabb.rs:114-125),
 // max = min + edge (aabb.rs:175-181).
@@ -59,6 +60,13 @@ __device__ __forceinline__ uint8_t sat_cube(const QueryGeom& g, const double (*a
     return rel;
 }
 
+// The node test of one location: In for AllPoints, s2_cube_relation for a cell union, else the separating-axis test.
+__device__ __forceinline__ uint8_t node_relation(const QueryGeom& g, const double (*aproj)[2], const double m[3], double e) {
+    if (g.kind == PCV_LOC_ALL) return REL_IN;
+    if (g.kind == kLocCellUnion) return (uint8_t)s2_cube_relation(m, e, g.squares, g.ncells);
+    return sat_cube(g, aproj, m, e);
+}
+
 __device__ __forceinline__ void project_location(const QueryGeom& g, double (*aproj)[2]) {
     for (int k = threadIdx.x; k < g.naxes; k += blockDim.x) {
         double lo = 1.7976931348623157e308, hi = -1.7976931348623157e308;
@@ -84,7 +92,7 @@ __global__ void __launch_bounds__(256) k_sat_nodes(const QueryGeom* __restrict__
     uint8_t r = REL_IN;
     if (g.kind != PCV_LOC_ALL) {
         const QNode nd = nodes[i];
-        r = sat_cube(g, aproj, nd.m, nd.e);
+        r = node_relation(g, aproj, nd.m, nd.e);
     }
     rel[(size_t)blockIdx.y * nnodes + i] = r;
 }
@@ -204,12 +212,32 @@ __device__ __forceinline__ bool loc_contains(const QueryGeom& g, double x, doubl
 }
 
 struct QTile {
-    uint32_t loc;
+    uint32_t loc;     // the location, | kTileIn when every point of the node passes its point test
     uint32_t node;
     uint32_t first;   // first point of the tile inside the node
     uint32_t count;
 };
 constexpr uint32_t kQueryTile = 2048;
+// Set on the tiles of a node a cell union classifies In: its points skip the point test (the interval filters still apply).
+constexpr uint32_t kTileIn = 0x80000000u;
+__host__ __device__ __forceinline__ uint32_t tile_loc(const QTile& t) { return t.loc & ~kTileIn; }
+
+// A cell union of at most kCellsShared ids is read from shared memory, staged once per tile; a larger one from global memory.
+constexpr uint32_t kCellsShared = 256;
+// The union's ids for the point test of one tile: staged into `sh` when they fit.  The caller synchronises the block before
+// the first read.
+__device__ __forceinline__ const uint64_t* stage_cells(const QueryGeom& g, uint64_t* sh) {
+    if (g.kind != kLocCellUnion || g.ncells > kCellsShared) return g.cells;
+    for (uint32_t k = threadIdx.x; k < g.ncells; k += blockDim.x) sh[k] = g.cells[k];
+    return sh;
+}
+
+// PointCulling::contains of the cull kernels: loc_contains, and for a cell union contains_cellid(from_point(p))
+// (s2_cell_union.rs:27-31) on the decoded position, over the union's ids at `cells`.
+__device__ __forceinline__ bool cull_contains(const QueryGeom& g, const uint64_t* cells, const double p[3]) {
+    if (g.kind == kLocCellUnion) return s2_union_contains(cells, g.ncells, s2_cell_id_from_point(p[0], p[1], p[2]));
+    return loc_contains(g, p[0], p[1], p[2]);
+}
 
 struct CullArgs {
     const QueryGeom* geoms;
@@ -242,9 +270,9 @@ __device__ __forceinline__ void decode_point(const uint8_t* xyz, const QNode& nd
     for (int k = 0; k < 3; ++k) p[k] = decode1_fast(load_code(s + k * bpc, nd.enc), nd.m[k], nd.e, nd.enc);  // == decode1, integer-built unit fraction
 }
 
-// PointCulling::contains, then the interval filters on the intensity of the point at `slot`.
-__device__ __forceinline__ bool point_passes(const CullArgs& a, const QueryGeom& g, const double p[3], uint64_t slot) {
-    bool keep = loc_contains(g, p[0], p[1], p[2]);
+// PointCulling::contains (skipped for a tile whose node is In), then the interval filters on the intensity of the point at `slot`.
+__device__ __forceinline__ bool point_passes(const CullArgs& a, const QueryGeom& g, const uint64_t* cells, bool all_in, const double p[3], uint64_t slot) {
+    bool keep = all_in || cull_contains(g, cells, p);
     if (a.nfilt) {
         const double v = (double)a.intensity[slot];  // iterator.rs:82-91: attribute as f64, closed interval
         for (uint32_t f = 0; f < a.nfilt; ++f) keep = keep && (a.filters[f].lo <= v && v <= a.filters[f].hi);
@@ -252,9 +280,10 @@ __device__ __forceinline__ bool point_passes(const CullArgs& a, const QueryGeom&
     return keep;
 }
 
-__device__ __forceinline__ bool eval_point(const CullArgs& a, const QueryGeom& g, const QNode& nd, uint32_t i, double p[3]) {
+__device__ __forceinline__ bool eval_point(const CullArgs& a, const QueryGeom& g, const uint64_t* cells, bool all_in, const QNode& nd, uint32_t i,
+                                           double p[3]) {
     decode_point(a.xyz, nd, enc_bytes(nd.enc), i, p);
-    return point_passes(a, g, p, nd.point_off + i);
+    return point_passes(a, g, cells, all_in, p, nd.point_off + i);
 }
 
 // The ordered cull of one tile per block: count pass (WRITE = false), then after k_scan_u32 the write pass.  SLOT = false: the
@@ -264,17 +293,20 @@ template <bool WRITE, bool SLOT>
 __device__ __forceinline__ void cull_tile(const CullArgs& a, const uint64_t* slot_base, uint64_t* out_slot) {
     __shared__ uint32_t warp_cnt[8];
     __shared__ uint32_t running;
+    __shared__ uint64_t scells[kCellsShared];
     const QTile t = a.tiles[blockIdx.x];
-    const QueryGeom& g = a.geoms[t.loc];
+    const QueryGeom& g = a.geoms[tile_loc(t)];
+    const bool all_in = (t.loc & kTileIn) != 0;
     const QNode nd = a.nodes[t.node];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint64_t* cells = stage_cells(g, scells);
     if (threadIdx.x == 0) running = WRITE ? a.tile_keep[blockIdx.x] : 0u;
     __syncthreads();
     for (uint32_t r0 = 0; r0 < t.count; r0 += 256) {
         const uint32_t i = r0 + threadIdx.x;
         double p[3] = {0, 0, 0};
         bool keep = false;
-        if (i < t.count) keep = eval_point(a, g, nd, t.first + i, p);
+        if (i < t.count) keep = eval_point(a, g, cells, all_in, nd, t.first + i, p);
         const unsigned bal = __ballot_sync(0xffffffffu, keep);
         if (lane == 0) warp_cnt[warp] = __popc(bal);
         __syncthreads();
@@ -387,8 +419,8 @@ __global__ void k_tile_totals(const QTile* tiles, const uint32_t* keep_counts, u
                               unsigned long long* tested) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= ntiles) return;
-    atomicAdd(&kept[tiles[i].loc], (unsigned long long)keep_counts[i]);
-    atomicAdd(&tested[tiles[i].loc], (unsigned long long)tiles[i].count);
+    atomicAdd(&kept[tile_loc(tiles[i])], (unsigned long long)keep_counts[i]);
+    atomicAdd(&tested[tile_loc(tiles[i])], (unsigned long long)tiles[i].count);
 }
 
 // ---- LOD draw order applied at build time (lod_order.h): gather every node's points into their shuffled order ------------------
@@ -476,12 +508,12 @@ __global__ void __launch_bounds__(256) k_bfs_level(const __grid_constant__ BfsAr
         const QueryGeom& g = a.geoms[pr.x];
         const QNode nd = a.nodes[pr.y];
         uint8_t rel = REL_IN;
-        if (g.kind != PCV_LOC_ALL) rel = sat_cube(g, a.proj[pr.x].a, nd.m, nd.e);
+        if (g.kind != PCV_LOC_ALL) rel = node_relation(g, a.proj[pr.x].a, nd.m, nd.e);
         if (rel == REL_OUT) continue;
         if (nd.n) {
             const uint32_t k = atomicAdd(a.npairs, 1u);
-            if (k < a.cap)
-                a.pairs[k] = pr;
+            if (k < a.cap)  // the pair's tiles carry kTileIn when a cell union holds the whole node
+                a.pairs[k] = make_uint2(g.kind == kLocCellUnion && rel == REL_IN ? (pr.x | kTileIn) : pr.x, pr.y);
             else
                 *a.overflow = 1;
             atomicAdd(a.ntiles, (unsigned long long)((nd.n + kQueryTileBfs - 1) / kQueryTileBfs));
@@ -557,11 +589,14 @@ __global__ void __launch_bounds__(256) k_cull_fused(const __grid_constant__ Cull
     __shared__ uint8_t st_rgb[256 * 3];
     __shared__ uint32_t wcnt[8];
     __shared__ unsigned long long sbase;
+    __shared__ uint64_t scells[kCellsShared];
     const CullArgs& a = f.c;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (uint32_t ti = blockIdx.x; ti < ntiles; ti += gridDim.x) {
         const QTile t = a.tiles[ti];
-        const QueryGeom& g = a.geoms[t.loc];
+        const uint32_t loc = tile_loc(t);
+        const QueryGeom& g = a.geoms[loc];
+        const bool all_in = (t.loc & kTileIn) != 0;
         const QNode nd = a.nodes[t.node];
         const bool staged = nd.enc != ENC_F64;
         const int bpc = enc_bytes(nd.enc);
@@ -570,6 +605,7 @@ __global__ void __launch_bounds__(256) k_cull_fused(const __grid_constant__ Cull
             const uint32_t nvec = (t.count * 3u * (uint32_t)bpc + 15u) >> 4;
             for (uint32_t v = threadIdx.x; v < nvec; v += 256) reinterpret_cast<uint4*>(sxyz)[v] = __ldcg(reinterpret_cast<const uint4*>(src) + v);
         }
+        const uint64_t* cells = stage_cells(g, scells);
         __syncthreads();
         uint32_t kept_tile = 0;  // thread 0 only
         for (uint32_t r0 = 0; r0 < t.count; r0 += 256) {
@@ -583,7 +619,7 @@ __global__ void __launch_bounds__(256) k_cull_fused(const __grid_constant__ Cull
 #pragma unroll
                     for (int k = 0; k < 3; ++k) p[k] = decode1_fast(load_code(src + ((size_t)i * 3 + k) * bpc, nd.enc), nd.m[k], nd.e, nd.enc);
                 }
-                keep = point_passes(a, g, p, nd.point_off + t.first + i);
+                keep = point_passes(a, g, cells, all_in, p, nd.point_off + t.first + i);
             }
             const unsigned bal = __ballot_sync(0xffffffffu, keep);
             if (lane == 0) wcnt[warp] = __popc(bal);
@@ -632,7 +668,7 @@ __global__ void __launch_bounds__(256) k_cull_fused(const __grid_constant__ Cull
             }
             __syncthreads();  // the staging arrays and wcnt are reused by the next round
         }
-        if (threadIdx.x == 0 && kept_tile) atomicAdd(&f.kept[t.loc], (unsigned long long)kept_tile);
+        if (threadIdx.x == 0 && kept_tile) atomicAdd(&f.kept[loc], (unsigned long long)kept_tile);
         __syncthreads();  // sxyz is reused by the next tile
     }
 }

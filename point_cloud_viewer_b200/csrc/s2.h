@@ -134,6 +134,120 @@ PCV_HD bool s2_union_intersects(const uint64_t* cells, uint32_t n, uint64_t id) 
     return i != 0 && s2_range_max(cells[i - 1]) >= s2_range_min(id);
 }
 
+// A cell as a face and the aligned square of leaf cells it covers: [i0, i0 + size) x [j0, j0 + size), size = 2^(30 - level).
+// A leaf cell lies in a cell iff its (face, i, j) lies in the cell's square (the curve subdivides the face as a quadtree).
+struct S2Square {
+    int32_t face;
+    uint32_t i0, j0, size;
+};
+
+// The inverse of s2_from_face_ij for a cell of any level: read its curve positions from the top, posToIJ per orientation.
+PCV_HD S2Square s2_to_face_ij_level(uint64_t id) {
+    S2Square q;
+    q.face = (int32_t)(id >> 61);
+    const int level = s2_level(id);
+    int orientation = q.face & 1;
+    uint32_t i = 0, j = 0;
+    for (int k = kS2MaxLevel - 1; k >= kS2MaxLevel - level; --k) {
+        const int pos = (int)((id >> (2 * k + 1)) & 3);
+        int ij;
+        switch (orientation) {
+            case 0: ij = pos == 0 ? 0 : pos == 1 ? 1 : pos == 2 ? 3 : 2; break;  // posToIJ[0] = {0, 1, 3, 2}
+            case 1: ij = pos == 0 ? 0 : pos == 1 ? 2 : pos == 2 ? 3 : 1; break;  // posToIJ[1] = {0, 2, 3, 1}
+            case 2: ij = pos == 0 ? 3 : pos == 1 ? 2 : pos == 2 ? 0 : 1; break;  // posToIJ[2] = {3, 2, 0, 1}
+            default: ij = pos == 0 ? 3 : pos == 1 ? 1 : pos == 2 ? 0 : 2; break; // posToIJ[3] = {3, 1, 0, 2}
+        }
+        i |= (uint32_t)(ij >> 1) << k;
+        j |= (uint32_t)(ij & 1) << k;
+        orientation ^= s2_pos_to_orientation(pos);
+    }
+    q.i0 = i;
+    q.j0 = j;
+    q.size = 1u << (kS2MaxLevel - level);
+    return q;
+}
+
+// The node test of a cell union: where the leaf cells s2_cell_id_from_point computes for the points of the cube [m, m + e]^3 can
+// lie, against the union's squares.  Out: no point's leaf cell is in the union; In: every point's is; Cross: otherwise.
+// Same coding as the query kernels' Relation (query.cuh).
+enum : int { kS2RelIn = 0, kS2RelCross = 1, kS2RelOut = 2 };
+
+// Soundness.  A point p of the cube with |p_k| <= 1e150 for every k and max |p_k| >= 1e-150 is normalised without over- or
+// underflow: x_n = RN(x * inv) with one inv for all three components, so the computed face has |p_a| >= |p_b| (1 - 2^-51) for its
+// axis a, and its u = RN(y_n / x_n) equals (y / x)(1 + d) with |d| < 2^-51 (inv cancels; three roundings), up to an absolute
+// 2^-1070 when y_n is subnormal.  The exact ratio of a cube point lies between the cube's extreme corner ratios, which are
+// computed here with one rounding each.  Widening every bound by the relative kS2Widen = 2^-40 and the absolute 1e-300 therefore
+// covers the point's computed u, v; s2_uv_to_st and s2_st_to_ij are monotone under correct rounding, so the widened bounds map to
+// bounds of its (i, j).  The same margin admits every face whose axis can come within 2^-40 of the largest component.  Cubes
+// outside that range (near the origin, huge or NaN corners) are Cross.  Decoded points lie in [m, RN(m + e)] (fma(t, e, m) with
+// 0 <= t <= 1), the cube tested here.
+constexpr double kS2Widen = 9.094947017729282e-13;  // 2^-40
+
+// v[k] with selects rather than an indexed load (a small array indexed at run time goes to a kernel's local memory)
+PCV_HD double s2_pick(const double v[3], int k) { return k == 0 ? v[0] : k == 1 ? v[1] : v[2]; }
+
+// [lo, hi] of N / D over N in [nlo, nhi] and D in [dlo, dhi], 0 < dlo: the extremes lie at the corners.
+PCV_HD void s2_ratio_bounds(double nlo, double nhi, double dlo, double dhi, double& lo, double& hi) {
+    const double a = nlo / dlo, b = nlo / dhi, c = nhi / dlo, d = nhi / dhi;
+    lo = a < b ? a : b;
+    hi = c > d ? c : d;
+    lo = lo - (fabs(lo) * kS2Widen + 1e-300);
+    hi = hi + (fabs(hi) * kS2Widen + 1e-300);
+    lo = lo < -1.0 ? -1.0 : lo;  // a computed u, v is in [-1, 1]: |y_n| <= |x_n| for the chosen face
+    hi = hi > 1.0 ? 1.0 : hi;
+}
+
+PCV_HD int s2_cube_relation(const double m[3], double e, const S2Square* sq, uint32_t n) {
+    if (n == 0) return kS2RelOut;
+    double lo[3], hi[3], amin[3];
+    bool near_origin = true;
+    for (int k = 0; k < 3; ++k) {
+        lo[k] = m[k];
+        hi[k] = m[k] + e;
+        if (!(fabs(lo[k]) <= 1e150 && fabs(hi[k]) <= 1e150 && lo[k] <= hi[k])) return kS2RelCross;
+        near_origin = near_origin && lo[k] <= 1e-150 && hi[k] >= -1e-150;
+        amin[k] = lo[k] > 0.0 ? lo[k] : hi[k] < 0.0 ? -hi[k] : 0.0;  // the smallest |p_k| over the cube
+    }
+    if (near_origin) return kS2RelCross;
+    // (u, v) of face f as (+-p_b / |p_a|, +-p_c / |p_a|): s2_face_uv's table with the sign of p_a folded in.  Packed (a nibble per
+    // face for b and c, a bit per face for a negative sign) so that no table lands in local memory:
+    //   b = {1, 0, 0, 2, 2, 1}, u negated on faces 1-4;  c = {2, 2, 1, 1, 0, 0}, v negated on faces 2-3
+    constexpr uint32_t kUAxis = 0x122001u, kUNeg = 0x1Eu, kVAxis = 0x001122u, kVNeg = 0x0Cu;
+    bool hit = false, all_in = true;
+    for (int f = 0; f < 6; ++f) {
+        const int a = f % 3;
+        const double dhi = f < 3 ? s2_pick(hi, a) : -s2_pick(lo, a);
+        if (!(dhi > 0.0)) continue;  // the major component of a point of this face has the face's sign
+        const double dl = f < 3 ? s2_pick(lo, a) : -s2_pick(hi, a), dlo = dl > 0.0 ? dl : 0.0;
+        const double reach = dhi + dhi * kS2Widen;
+        if (reach < s2_pick(amin, (a + 1) % 3) || reach < s2_pick(amin, (a + 2) % 3)) continue;  // p_a is never the largest component
+        double ulo = -1.0, uhi = 1.0, vlo = -1.0, vhi = 1.0;
+        if (dlo >= 1e-150) {
+            const int b = (int)((kUAxis >> (4 * f)) & 15u), c = (int)((kVAxis >> (4 * f)) & 15u);
+            const bool un = (kUNeg >> f) & 1u, vn = (kVNeg >> f) & 1u;
+            const double blo = s2_pick(lo, b), bhi = s2_pick(hi, b), clo = s2_pick(lo, c), chi = s2_pick(hi, c);
+            s2_ratio_bounds(un ? -bhi : blo, un ? -blo : bhi, dlo, dhi, ulo, uhi);
+            s2_ratio_bounds(vn ? -chi : clo, vn ? -clo : chi, dlo, dhi, vlo, vhi);
+        }
+        const uint32_t i0 = (uint32_t)s2_st_to_ij(s2_uv_to_st(ulo)), i1 = (uint32_t)s2_st_to_ij(s2_uv_to_st(uhi));
+        const uint32_t j0 = (uint32_t)s2_st_to_ij(s2_uv_to_st(vlo)), j1 = (uint32_t)s2_st_to_ij(s2_uv_to_st(vhi));
+        bool face_hit = false, covered = false;
+        for (uint32_t k = 0; k < n; ++k) {
+            const S2Square s = sq[k];
+            const uint32_t ie = s.i0 + (s.size - 1), je = s.j0 + (s.size - 1);  // last leaf row / column of the square
+            if (s.face != f || i1 < s.i0 || i0 > ie || j1 < s.j0 || j0 > je) continue;
+            face_hit = true;
+            if (i0 >= s.i0 && i1 <= ie && j0 >= s.j0 && j1 <= je) {
+                covered = true;
+                break;
+            }
+        }
+        hit = hit || face_hit;
+        all_in = all_in && covered;
+    }
+    return !hit ? kS2RelOut : all_in ? kS2RelIn : kS2RelCross;
+}
+
 // The S2Splitter's validity rule (read_write/s2.rs:64-71): |p| outside [EARTH_RADIUS_MIN_M, EARTH_RADIUS_MAX_M] is an error.
 // nalgebra's norm(): sqrt of the sum of squares in x, y, z order.
 PCV_HD bool s2_valid_ecef(double x, double y, double z) {

@@ -15,6 +15,7 @@ import math
 
 import numpy as np
 
+from ._native import CellUnion as _NativeCellUnion
 from ._native import Location
 
 LOC_ALL, LOC_AABB, LOC_FRUSTUM, LOC_OBB = 0, 1, 2, 3
@@ -163,6 +164,23 @@ def obb(query_from_obb, half_extent):
     loc.obb_from_query[:] = query_from_obb.inverse().as7()
     loc.half_extent[:] = [float(v) for v in half_extent]
     return loc
+
+
+class CellUnion:
+    """PointLocation::S2Cells (src/iterator.rs:13-20): the points whose leaf cell the union of S2 cells `ids` contains.  Not a
+    pcv_location: Octree / OctreeDir queries dispatch it to the pcv_*cell_union* entry points, which validate and normalise the
+    ids."""
+
+    def __init__(self, ids):
+        self.ids = np.ascontiguousarray(np.asarray(ids, np.uint64).reshape(-1))
+
+    def struct(self):
+        """The pcv_cell_union view of the ids (valid while this object lives)."""
+        return _NativeCellUnion(self.ids.ctypes.data if len(self.ids) else None, len(self.ids), 0)
+
+
+def cell_union(ids):
+    return CellUnion(ids)
 
 
 def obb_from_aabb(mins, maxs):
