@@ -398,6 +398,28 @@ int pcv_s2_cells_in_union(const pcv_s2cloud* cloud, const uint64_t* union_ids, u
  * input order inside a cell.  n_out = number of survivors (may exceed cap: only cap are written). */
 int pcv_s2_query_union(const pcv_s2cloud* cloud, const uint64_t* union_ids, uint32_t n_union, double* xyz_out, uint8_t* rgb_out,
                        float* intensity_out, uint64_t* src_index_out, uint64_t cap, uint64_t* n_out, uint64_t* tested_out);
+/* Every PointLocation except WebMercatorRect, with interval filters, streamed or batched on the GPU.  A cell's point box is the
+ * exact component-wise min and max of its stored positions.  AllPoints selects every cell; Aabb, Obb and Frustum select the
+ * cells whose point box the location's separating-axis test (cache_separating_axes_for_aabb, sat.rs) does not call Out (a cell
+ * without points has no box and is never selected); a cell union selects the cells whose id range intersects it.  This cell
+ * list is not the reference's (which selects through latitude / longitude rectangles); the points are a superset of the
+ * reference's: every point of a selected cell that passes PointCulling::contains and every filter interval (intensity as f64,
+ * closed).  Points come in cell (id) order, input order inside a cell; positions are the stored doubles, rgb is NULL for a
+ * cloud without colour, src_index is the build input index (the slot for a loaded directory).
+ * pcv_s2_cells_in_location: the selected cells in id order (AllPoints: every cell); ids_out may be NULL to count, n_out may
+ * exceed cap (only cap are written).  The stream and batch calls behave like pcv_query_points / pcv_query_batch_device
+ * (batches of exactly batch_size points but the last, PCV_ERR_CANCELLED when the callback stops, filters on a cloud without
+ * intensity are PCV_ERR_INVALID) and fill pcv_last_query_stats the same way; their algorithmic_bytes are 24 B per tested
+ * position (+ 4 B of intensity with filters) plus every survivor's position, colour and intensity. */
+int pcv_s2_cells_in_location(const pcv_s2cloud* cloud, const pcv_location* loc, uint64_t* ids_out, uint64_t cap, uint64_t* n_out);
+int pcv_s2_query_points(const pcv_s2cloud* cloud, const pcv_location* loc, const pcv_interval* filters, uint32_t nfilt,
+                        uint64_t batch_size, pcv_batch_cb cb, void* user);
+int pcv_s2_query_cell_union(const pcv_s2cloud* cloud, const pcv_cell_union* cu, const pcv_interval* filters, uint32_t nfilt,
+                            uint64_t batch_size, pcv_batch_cb cb, void* user);
+int pcv_s2_query_batch_device(const pcv_s2cloud* cloud, const pcv_location* locs, uint32_t nloc, const pcv_interval* filters,
+                              uint32_t nfilt, uint64_t* counts_out, uint64_t* tested_out);
+int pcv_s2_query_cell_unions_batch_device(const pcv_s2cloud* cloud, const pcv_cell_union* unions, uint32_t nunion,
+                                          const pcv_interval* filters, uint32_t nfilt, uint64_t* counts_out, uint64_t* tested_out);
 /* The directory an S2Splitter<RawNodeWriter> leaves behind (read_write/s2.rs:127-145, raw.rs): per cell `<to_token()>.xyz`
  * (f64 LE x, y, z), `.rgb`, `.intensity`, and meta.pb = Meta { version 13, bounding_box, s2 { cells, attributes } }
  * (s2_cells/mod.rs:77-104); load = S2Cells::from_data_provider over such a directory (:106-147, :203-216; versions < 12 and

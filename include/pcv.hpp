@@ -291,10 +291,10 @@ class Octree {
 inline PointsBatch batch_from(const pcv_batch* b) {
     PointsBatch pb;
     pb.position.resize(b->n);
-    pb.color.resize(b->n);
+    if (b->rgb) pb.color.resize(b->n);  // an S2 cloud without colour delivers none
     for (uint64_t i = 0; i < b->n; ++i) {
         pb.position[i] = {b->xyz[3 * i], b->xyz[3 * i + 1], b->xyz[3 * i + 2]};
-        pb.color[i] = {b->rgb[3 * i], b->rgb[3 * i + 1], b->rgb[3 * i + 2]};
+        if (b->rgb) pb.color[i] = {b->rgb[3 * i], b->rgb[3 * i + 1], b->rgb[3 * i + 2]};
     }
     if (b->intensity) pb.intensity.assign(b->intensity, b->intensity + b->n);
     pb.source_index.assign(b->src_index, b->src_index + b->n);
@@ -561,12 +561,56 @@ class S2Cells {
                                      nullptr));
         return b;
     }
+    // PointCloud::nodes_in_location for AllPoints, Aabb, Obb and Frustum: the cells whose point box the location's separating-axis
+    // test does not call Out, in id order (not the reference's rectangle-based list; see pcv_s2_cells_in_location)
+    std::vector<CellID> nodes_in_location(const PointLocation& loc) const {
+        uint64_t n = 0;
+        check(pcv_s2_cells_in_location(s_, &loc.raw, nullptr, 0, &n));
+        std::vector<CellID> out(n);
+        check(pcv_s2_cells_in_location(s_, &loc.raw, out.data(), n, &n));
+        return out;
+    }
+    // PointQuery streamed in batches of `batch_size` points (the last one short), in cell order; func returns false to stop.
+    // Returns true if every batch was consumed.  `color` is empty for a cloud without colour.
+    bool for_each_batch(const PointQuery& query, size_t batch_size, const std::function<bool(PointsBatch&&)>& func) const;
+    // The points of PointLocation::S2Cells(cell_union) that pass the filter intervals, in cell order
+    bool for_each_batch(const CellUnion& cell_union, const std::vector<ClosedInterval>& filter_intervals, size_t batch_size,
+                        const std::function<bool(PointsBatch&&)>& func) const;
+    // survivors and tested points of every location / cell union
+    void query_batch(const std::vector<PointLocation>& locs, std::vector<uint64_t>& counts, std::vector<uint64_t>& tested) const {
+        std::vector<pcv_location> raw;
+        for (auto& l : locs) raw.push_back(l.raw);
+        counts.assign(locs.size(), 0);
+        tested.assign(locs.size(), 0);
+        check(pcv_s2_query_batch_device(s_, raw.data(), (uint32_t)raw.size(), nullptr, 0, counts.data(), tested.data()));
+    }
+    void query_batch(const std::vector<CellUnion>& unions, std::vector<uint64_t>& counts, std::vector<uint64_t>& tested) const {
+        const std::vector<pcv_cell_union> raw = detail::raw_unions(unions);
+        counts.assign(unions.size(), 0);
+        tested.assign(unions.size(), 0);
+        check(pcv_s2_query_cell_unions_batch_device(s_, raw.data(), (uint32_t)raw.size(), nullptr, 0, counts.data(), tested.data()));
+    }
     void write_to_directory(const std::string& dir) const { check(pcv_s2_write_dir(s_, dir.c_str())); }
     pcv_s2cloud* raw() const { return s_; }
 
    private:
     pcv_s2cloud* s_;
 };
+
+inline bool S2Cells::for_each_batch(const PointQuery& query, size_t batch_size, const std::function<bool(PointsBatch&&)>& func) const {
+    const std::vector<pcv_interval> f = detail::raw_intervals(query.filter_intervals);
+    return detail::stream_batches(func, [&](pcv_batch_cb cb, void* user) {
+        return pcv_s2_query_points(s_, &query.location.raw, f.empty() ? nullptr : f.data(), (uint32_t)f.size(), batch_size, cb, user);
+    });
+}
+inline bool S2Cells::for_each_batch(const CellUnion& cell_union, const std::vector<ClosedInterval>& filter_intervals, size_t batch_size,
+                                    const std::function<bool(PointsBatch&&)>& func) const {
+    const pcv_cell_union cu = detail::raw_union(cell_union);
+    const std::vector<pcv_interval> f = detail::raw_intervals(filter_intervals);
+    return detail::stream_batches(func, [&](pcv_batch_cb cb, void* user) {
+        return pcv_s2_query_cell_union(s_, &cu, f.empty() ? nullptr : f.data(), (uint32_t)f.size(), batch_size, cb, user);
+    });
+}
 
 // S2Splitter::with_split_level(level, path, Encoding::Plain, ..) + write(batch)... + get_meta (read_write/s2.rs:33-50,59-125,165-173):
 // the batches of one cloud, split by S2 cell on the GPU; throws ("... is not a valid ECEF point") like the writer's Err.

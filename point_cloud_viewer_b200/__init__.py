@@ -683,7 +683,7 @@ def _query_points(fn, h, loc, callback, filters, batch_size):
         n = b.n
         d = dict(
             xyz=np.ctypeslib.as_array(C.cast(b.xyz, C.POINTER(C.c_double)), (n, 3)).copy() if n else np.zeros((0, 3)),
-            rgb=np.ctypeslib.as_array(C.cast(b.rgb, C.POINTER(C.c_uint8)), (n, 3)).copy() if n else np.zeros((0, 3), np.uint8),
+            rgb=None if not b.rgb else np.ctypeslib.as_array(C.cast(b.rgb, C.POINTER(C.c_uint8)), (n, 3)).copy() if n else np.zeros((0, 3), np.uint8),
             intensity=np.ctypeslib.as_array(C.cast(b.intensity, C.POINTER(C.c_float)), (n,)).copy() if (n and b.intensity) else None,
             src=np.ctypeslib.as_array(C.cast(b.src_index, C.POINTER(C.c_uint64)), (n,)).copy() if n else np.zeros(0, np.uint64),
         )
@@ -854,6 +854,32 @@ class S2Cloud:
         N.check(N.lib().pcv_s2_query_union(self.h, _p(u), nu, _p(xyz), _p(rgb), _p(inten), _p(src), cap, C.byref(n), C.byref(tested)))
         m = min(cap, n.value)
         return dict(xyz=xyz[:m], rgb=None if rgb is None else rgb[:m], intensity=None if inten is None else inten[:m], src=src[:m], total=n.value, tested=tested.value)
+
+    def cells_in_location(self, loc):
+        """nodes_in_location for any location: a pcv_location (the cells whose point box the location's separating-axis test
+        does not call Out, in id order; AllPoints: every cell) or a geometry.CellUnion (cells_in_union)."""
+        if isinstance(loc, geometry.CellUnion):  # an empty union selects no cell (None would mean AllPoints)
+            return self.cells_in_union(loc.ids) if len(loc.ids) else np.zeros(0, np.uint64)
+        out = np.zeros(max(self.num_cells, 1), np.uint64)
+        n = C.c_uint64()
+        N.check(N.lib().pcv_s2_cells_in_location(self.h, C.byref(loc), _p(out), self.num_cells, C.byref(n)))
+        return out[: n.value]
+
+    def query_points(self, loc, callback=None, filters=(), batch_size=500000):
+        """Octree.query_points over the cloud: batches dict(xyz, rgb (None without colour), intensity, src) of the points of the
+        selected cells that pass the location's point test and the filter intervals, in cell order."""
+        fn = N.lib().pcv_s2_query_cell_union if isinstance(loc, geometry.CellUnion) else N.lib().pcv_s2_query_points
+        return _query_points(fn, self.h, loc, callback, filters, batch_size)
+
+    def query_batch_device(self, locs, filters=()):
+        """(counts, tested) per location, as Octree.query_batch_device; the locations are all pcv_locations or all geometry.CellUnions."""
+        return _query_batch(N.lib().pcv_s2_query_batch_device, N.lib().pcv_s2_query_cell_unions_batch_device, self.h, locs, filters)
+
+    def last_query_stats(self):
+        """Timing / traffic of the last query_batch_device call on the context (pcv_query_stats)."""
+        st = N.QueryStats()
+        N.check(N.lib().pcv_last_query_stats(self.ctx.h, C.byref(st)))
+        return {k: getattr(st, k) for k, _ in N.QueryStats._fields_}
 
 
 def s2_token(cell_id):

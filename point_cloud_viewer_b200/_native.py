@@ -255,6 +255,11 @@ SYMBOLS = [
     ("pcv_s2_cell_data", C.c_int, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("pcv_s2_cells_in_union", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, _u64p]),
     ("pcv_s2_query_union", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, _u64p, _u64p]),
+    ("pcv_s2_cells_in_location", C.c_int, [C.c_void_p, C.POINTER(Location), C.c_void_p, C.c_uint64, _u64p]),
+    ("pcv_s2_query_points", C.c_int, [C.c_void_p, C.POINTER(Location), C.c_void_p, C.c_uint32, C.c_uint64, BATCH_CB, C.c_void_p]),
+    ("pcv_s2_query_cell_union", C.c_int, [C.c_void_p, C.POINTER(CellUnion), C.c_void_p, C.c_uint32, C.c_uint64, BATCH_CB, C.c_void_p]),
+    ("pcv_s2_query_batch_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
+    ("pcv_s2_query_cell_unions_batch_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
     ("pcv_s2_write_dir", C.c_int, [C.c_void_p, C.c_char_p]),
     ("pcv_s2_load_dir", C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),
     ("pcv_s2_union_contains", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_void_p, C.c_uint32, C.c_void_p]),

@@ -192,6 +192,42 @@ inline QueryGeom make_query_geom(const pcv_location& loc) {
     return g;
 }
 
+// The separating-axis test of a location against an arbitrary box [mn, mx] (the point box of an S2 cell, s2_api.inl): sat()
+// of sat.rs:174-194 over the location's cached axes, the box's 8 corners in the Aabb order (x fastest, aabb.rs:114-125), exactly
+// as sat_cube (query.cuh) tests a node cube, whose max is min + edge.  Shared by the device kernels and the test backend.
+// project_location_axis: the location's own projection on axis k (project_location of query.cuh, one axis).
+PCV_GHD void project_location_axis(const QueryGeom& g, int k, double& lo, double& hi) {
+    lo = 1.7976931348623157e308;
+    hi = -1.7976931348623157e308;
+    for (int i = 0; i < 8; ++i) {
+        const double p = g.corners[i][0] * g.axes[k][0] + g.corners[i][1] * g.axes[k][1] + g.corners[i][2] * g.axes[k][2];
+        lo = fmin(lo, p);
+        hi = fmax(hi, p);
+    }
+}
+PCV_GHD void project_box(const double mn[3], const double mx[3], const double ax[3], double& lo, double& hi) {
+    lo = 1.7976931348623157e308;
+    hi = -1.7976931348623157e308;
+    for (int i = 0; i < 8; ++i) {
+        const double cx = (i & 1) ? mx[0] : mn[0], cy = (i & 2) ? mx[1] : mn[1], cz = (i & 4) ? mx[2] : mn[2];
+        const double p = cx * ax[0] + cy * ax[1] + cz * ax[2];
+        lo = fmin(lo, p);
+        hi = fmax(hi, p);
+    }
+}
+// kS2RelIn / kS2RelCross / kS2RelOut; aproj[k] = project_location_axis(g, k)
+PCV_GHD int sat_box(const QueryGeom& g, const double (*aproj)[2], const double mn[3], const double mx[3]) {
+    int rel = kS2RelIn;
+    for (int k = 0; k < g.naxes; ++k) {
+        double bmin, bmax;
+        project_box(mn, mx, g.axes[k], bmin, bmax);
+        const double amin = aproj[k][0], amax = aproj[k][1];
+        if (bmin > amax || bmax < amin) return kS2RelOut;
+        if (amin > bmin || bmax > amax) rel = kS2RelCross;
+    }
+    return rel;
+}
+
 // The location of an X-ray tile with box [tmin, tmax]: Aabb(bbox), or Obb::from(bbox).transformed(query_from_global.inverse())
 // (xray generation.rs:471-477).
 inline pcv_location xray_location(const double tmin[3], const double tmax[3], const double* qfg) {

@@ -6,6 +6,7 @@
 //   k_cull<0/1>, k_cull_chunk<0/1>  a13-a15  decode + PointCulling::contains + interval filters + order-preserving
 //                                   count / write passes (FilteredIterator, iterator.rs:96-119)
 //   k_cull_fused<0/1>               a13-a15  the same test in one pass: batched counts, with (1) or without (0) the survivors
+//   k_s2_cell_boxes, k_s2_select_cells      the S2 cloud's point boxes and cell selection; its cells are culled by the kernels above
 //   k_xray_bin<0/1>, k_xray_subtile a19  discretise + per-pixel 1024-bit z-bucket set + grey mapping
 //
 // All arithmetic is binary64 in the reference's operation order (compiled with -fmad=false).
@@ -59,6 +60,8 @@ __device__ __forceinline__ uint8_t sat_cube(const QueryGeom& g, const double (*a
     }
     return rel;
 }
+
+// The same test against an arbitrary box (an S2 cell's point box) is sat_box of geometry_host.hpp, shared with the test backend.
 
 // The node test of one location: In for AllPoints, s2_cube_relation for a cell union, else the separating-axis test.
 __device__ __forceinline__ uint8_t node_relation(const QueryGeom& g, const double (*aproj)[2], const double m[3], double e) {
@@ -288,8 +291,9 @@ __device__ __forceinline__ bool eval_point(const CullArgs& a, const QueryGeom& g
 
 // The ordered cull of one tile per block: count pass (WRITE = false), then after k_scan_u32 the write pass.  SLOT = false: the
 // survivor's provenance is gathered from the resident `src` array (k_cull); SLOT = true: it is the point's slot in the node table,
-// slot_base[piece] + first + i (k_cull_chunk, for pieces of nodes streamed from disk).
-template <bool WRITE, bool SLOT>
+// slot_base[piece] + first + i (k_cull_chunk, for pieces of nodes streamed from disk).  RGB = false: the cloud has no colour
+// (an S2 cloud may have none; an octree always has it), rgb / out_rgb are not touched.
+template <bool WRITE, bool SLOT, bool RGB = true>
 __device__ __forceinline__ void cull_tile(const CullArgs& a, const uint64_t* slot_base, uint64_t* out_slot) {
     __shared__ uint32_t warp_cnt[8];
     __shared__ uint32_t running;
@@ -323,9 +327,11 @@ __device__ __forceinline__ void cull_tile(const CullArgs& a, const uint64_t* slo
             a.out_xyz[3 * dst] = p[0];
             a.out_xyz[3 * dst + 1] = p[1];
             a.out_xyz[3 * dst + 2] = p[2];
-            a.out_rgb[3 * dst] = a.rgb[3 * sp];
-            a.out_rgb[3 * dst + 1] = a.rgb[3 * sp + 1];
-            a.out_rgb[3 * dst + 2] = a.rgb[3 * sp + 2];
+            if (RGB) {
+                a.out_rgb[3 * dst] = a.rgb[3 * sp];
+                a.out_rgb[3 * dst + 1] = a.rgb[3 * sp + 1];
+                a.out_rgb[3 * dst + 2] = a.rgb[3 * sp + 2];
+            }
             if (a.out_intensity) a.out_intensity[dst] = a.intensity[sp];
             if (SLOT)
                 out_slot[dst] = slot_base[t.node] + t.first + i;
@@ -338,9 +344,9 @@ __device__ __forceinline__ void cull_tile(const CullArgs& a, const uint64_t* slo
     }
     if (!WRITE && threadIdx.x == 0) a.tile_keep[blockIdx.x] = running;
 }
-template <bool WRITE>
+template <bool WRITE, bool RGB = true>
 __global__ void __launch_bounds__(256) k_cull(const __grid_constant__ CullArgs a) {
-    cull_tile<WRITE, false>(a, nullptr, nullptr);
+    cull_tile<WRITE, false, RGB>(a, nullptr, nullptr);
 }
 // One chunk of a directory-backed query: `nodes` / `tiles` are the chunk's pieces (chunk-local offsets), `src` / `out_src` unused.
 struct CullChunkArgs {
@@ -550,6 +556,114 @@ __global__ void __launch_bounds__(256) k_pairs_to_tiles(const uint2* __restrict_
     }
 }
 
+// ---- S2 cells: location queries of an S2 cloud (s2_api.inl) -------------------------------------------------------------------
+// The cells of an S2 cloud go to the cull kernels as Float64 nodes (QNode m = -0.0, e = 1: fma(v, 1, -0.0) == v for every v, so
+// the decoded position is the stored double, bit for bit).  A cell is selected by the separating-axis test of the location
+// against its point box: the exact component-wise min and max of its stored positions.
+//
+// k_s2_cell_boxes: the point boxes, one block per work tile (cell, first, count) of the cell-contiguous positions.  Min and max
+// are taken over order-preserving integer keys of the doubles (warp shuffles, then one atomic per warp and bound), so the box
+// does not depend on the order in which tiles and lanes meet; k_s2_box_keys_to_f64 turns the keys back into doubles.
+__device__ __forceinline__ unsigned long long f64_order_key(double v) {
+    const unsigned long long u = (unsigned long long)__double_as_longlong(v);
+    return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
+}
+__device__ __forceinline__ double f64_from_order_key(unsigned long long k) {
+    return __longlong_as_double((long long)((k >> 63) ? (k & 0x7FFFFFFFFFFFFFFFull) : ~k));
+}
+// kmin / kmax: [cell * 3 + axis], preset to ~0 / 0
+__global__ void __launch_bounds__(256) k_s2_cell_boxes(const double* __restrict__ xyz, const QNode* __restrict__ cells, const QTile* __restrict__ tiles,
+                                                      uint32_t ntiles, unsigned long long* __restrict__ kmin, unsigned long long* __restrict__ kmax) {
+    for (uint32_t ti = blockIdx.x; ti < ntiles; ti += gridDim.x) {
+        const QTile t = tiles[ti];
+        const uint64_t first = cells[t.node].point_off + t.first;
+        unsigned long long lo[3] = {~0ull, ~0ull, ~0ull}, hi[3] = {0ull, 0ull, 0ull};
+        for (uint32_t i = threadIdx.x; i < t.count; i += blockDim.x) {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                const unsigned long long key = f64_order_key(__ldcs(xyz + 3 * (first + i) + k));
+                lo[k] = min(lo[k], key);
+                hi[k] = max(hi[k], key);
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                lo[k] = min(lo[k], __shfl_xor_sync(0xffffffffu, lo[k], o));
+                hi[k] = max(hi[k], __shfl_xor_sync(0xffffffffu, hi[k], o));
+            }
+        if ((threadIdx.x & 31) == 0 && threadIdx.x < t.count)
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                atomicMin(&kmin[3 * (size_t)t.node + k], lo[k]);
+                atomicMax(&kmax[3 * (size_t)t.node + k], hi[k]);
+            }
+    }
+}
+__global__ void __launch_bounds__(256) k_s2_box_keys_to_f64(unsigned long long* __restrict__ keys, size_t n) {
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const double v = f64_from_order_key(keys[i]);
+        reinterpret_cast<double*>(keys)[i] = v;
+    }
+}
+
+// k_s2_select_cells: grid (cells / 256, locations).  Every thread tests one (location, cell): AllPoints selects every cell, a cell
+// union the cells its ranges intersect (In when the union contains the whole cell: its points skip the point test), any other
+// location the cells whose point box sat_box does not call Out.  A selected cell with points joins the pair list (no
+// particular order); its tiles and points are added to ntiles and tested[location].  The pair list holds nloc * ncells entries:
+// it cannot overflow.
+struct S2SelectArgs {
+    const QueryGeom* geoms;
+    const LocProj* proj;
+    const QNode* cells;
+    const uint64_t* ids;
+    const double* bmin;       // [cell * 3 + axis] point boxes
+    const double* bmax;
+    uint32_t ncells;
+    uint2* pairs;             // (location | kTileIn, cell)
+    uint32_t* npairs;
+    unsigned long long* ntiles;
+    unsigned long long* tested;  // [location]
+};
+__global__ void __launch_bounds__(256) k_s2_select_cells(const __grid_constant__ S2SelectArgs a) {
+    __shared__ double aproj[26][2];
+    const uint32_t loc = blockIdx.y;
+    const QueryGeom& g = a.geoms[loc];
+    for (int k = threadIdx.x; k < 52; k += blockDim.x) aproj[k >> 1][k & 1] = a.proj[loc].a[k >> 1][k & 1];
+    __syncthreads();
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int lane = threadIdx.x & 31;
+    uint32_t n = 0, flag = 0;
+    if (i < a.ncells) {
+        int rel = kS2RelIn;
+        if (g.kind == kLocCellUnion) {
+            const uint64_t id = a.ids[i];
+            rel = !s2_union_intersects(g.cells, g.ncells, id) ? kS2RelOut : s2_union_contains(g.cells, g.ncells, id) ? kS2RelIn : kS2RelCross;
+            if (rel == kS2RelIn) flag = kTileIn;
+        } else if (g.kind != PCV_LOC_ALL) {
+            rel = sat_box(g, aproj, a.bmin + 3 * (size_t)i, a.bmax + 3 * (size_t)i);
+        }
+        if (rel != kS2RelOut) n = a.cells[i].n;
+    }
+    const unsigned sel = __ballot_sync(0xffffffffu, n != 0);
+    if (sel == 0) return;
+    uint32_t base = 0;
+    if (lane == 0) base = atomicAdd(a.npairs, (uint32_t)__popc(sel));
+    base = __shfl_sync(0xffffffffu, base, 0);
+    if (n) a.pairs[base + __popc(sel & ((1u << lane) - 1u))] = make_uint2(loc | flag, i);
+    unsigned long long nt = (n + kQueryTile - 1) / kQueryTile, np = n;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        nt += __shfl_xor_sync(0xffffffffu, nt, o);
+        np += __shfl_xor_sync(0xffffffffu, np, o);
+    }
+    if (lane == 0) {
+        atomicAdd(a.ntiles, nt);
+        atomicAdd(&a.tested[loc], np);
+    }
+}
+
 // FilteredIterator (iterator.rs:96-119) over one tile, in ONE pass: the tile's position bytes are staged in shared memory with
 // 16-byte loads (node blocks and 2048-point tiles are 16-byte aligned), every point is decoded and tested once; per round of
 // 256 points the block counts its survivors with ballots, reserves their output range with one atomic, stages them in shared
@@ -579,7 +693,8 @@ __device__ __forceinline__ void decode_staged(const uint8_t* s, uint32_t i, cons
         for (int k = 0; k < 3; ++k) p[k] = decode_axis<ENC_F32>(q[k], nd.m[k], nd.e);
     }
 }
-template <bool STORE>
+// RGB = false (STORE only): the cloud has no colour, rgb / out_rgb are not touched (as in cull_tile).
+template <bool STORE, bool RGB = true>
 __global__ void __launch_bounds__(256) k_cull_fused(const __grid_constant__ CullFusedArgs f, uint32_t ntiles) {
     __shared__ __align__(16) uint8_t sxyz[kCullStage];
     // survivors of one round of 256 points, staged so that the copy-out is contiguous 8 / 4 / 1-byte-per-lane stores
@@ -651,9 +766,11 @@ __global__ void __launch_bounds__(256) k_cull_fused(const __grid_constant__ Cull
                 st_xyz[3 * li] = p[0];
                 st_xyz[3 * li + 1] = p[1];
                 st_xyz[3 * li + 2] = p[2];
-                st_rgb[3 * li] = a.rgb[3 * sp];
-                st_rgb[3 * li + 1] = a.rgb[3 * sp + 1];
-                st_rgb[3 * li + 2] = a.rgb[3 * sp + 2];
+                if (RGB) {
+                    st_rgb[3 * li] = a.rgb[3 * sp];
+                    st_rgb[3 * li + 1] = a.rgb[3 * sp + 1];
+                    st_rgb[3 * li + 2] = a.rgb[3 * sp + 2];
+                }
                 st_src[li] = a.src[sp];
                 if (a.out_intensity) st_int[li] = a.intensity[sp];
             }
@@ -661,7 +778,8 @@ __global__ void __launch_bounds__(256) k_cull_fused(const __grid_constant__ Cull
             const unsigned long long base = sbase;
             const uint32_t room = base >= f.cap ? 0u : (uint32_t)min((unsigned long long)total, f.cap - base);
             for (uint32_t k = threadIdx.x; k < 3 * room; k += 256) a.out_xyz[3 * base + k] = st_xyz[k];
-            for (uint32_t k = threadIdx.x; k < 3 * room; k += 256) a.out_rgb[3 * base + k] = st_rgb[k];
+            if (RGB)
+                for (uint32_t k = threadIdx.x; k < 3 * room; k += 256) a.out_rgb[3 * base + k] = st_rgb[k];
             for (uint32_t k = threadIdx.x; k < room; k += 256) {
                 a.out_src[base + k] = st_src[k];
                 if (a.out_intensity) a.out_intensity[base + k] = st_int[k];
