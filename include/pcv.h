@@ -151,7 +151,10 @@ int pcv_visible_nodes(const pcv_octree* o, const double clip_from_world[16], uin
 
 /* ---- a15-a16: PointQuery streaming (iterator.rs:66-119,255-333) ----------------------------- */
 /* Streams every point of every node in `loc` that passes the culling + interval filters, re-chunked
- * into batches of exactly batch_size points (last one short), on the caller's thread. */
+ * into batches of exactly batch_size points (last one short), on the caller's thread.
+ * The argument contract holds for all three sources (octree, octree directory, S2 cloud) and their nodes / cells, stream and
+ * batch calls: a location kind outside PCV_LOC_ALL..PCV_LOC_OBB, nfilt > 0 with filters == NULL, or filters over points
+ * without intensity is PCV_ERR_INVALID; a callback that returns non-zero ends the stream with PCV_ERR_CANCELLED. */
 int pcv_query_points(const pcv_octree* o, const pcv_location* loc, const pcv_interval* filters, uint32_t nfilt,
                      uint64_t batch_size, pcv_batch_cb cb, void* user);
 /* Throughput form: nloc locations in one call; survivors stay compacted in HBM.  counts_out[i] =

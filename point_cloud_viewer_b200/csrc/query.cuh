@@ -396,39 +396,6 @@ __global__ void __launch_bounds__(1024) k_scan_u32(uint32_t* v, uint32_t n, unsi
     if (threadIdx.x == 0) *total_out = carry;
 }
 
-// Work list of the batched query: one QTile per kQueryTile points of every (location, node) pair that passed.
-// The order of the list is irrelevant for the batched form (only per-location totals and the compacted survivors
-// are produced), so tiles are appended with one atomic per pair.
-__global__ void __launch_bounds__(256) k_count_tiles(const uint8_t* __restrict__ pass, const QNode* __restrict__ nodes, uint32_t nnodes,
-                                                     uint64_t npairs, unsigned long long* __restrict__ total) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    unsigned long long c = 0;
-    if (i < npairs && pass[i]) c = (nodes[i % nnodes].n + kQueryTile - 1) / kQueryTile;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-    if ((threadIdx.x & 31) == 0 && c) atomicAdd(total, c);
-}
-__global__ void __launch_bounds__(256) k_fill_tiles(const uint8_t* __restrict__ pass, const QNode* __restrict__ nodes, uint32_t nnodes,
-                                                    uint64_t npairs, unsigned long long* __restrict__ cursor, QTile* __restrict__ tiles) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= npairs || !pass[i]) return;
-    const uint32_t node = (uint32_t)(i % nnodes), loc = (uint32_t)(i / nnodes);
-    const uint32_t n = nodes[node].n;
-    if (n == 0) return;
-    const uint32_t nt = (n + kQueryTile - 1) / kQueryTile;
-    const unsigned long long base = atomicAdd(cursor, (unsigned long long)nt);
-    for (uint32_t k = 0; k < nt; ++k) tiles[base + k] = QTile{loc, node, k * kQueryTile, min(kQueryTile, n - k * kQueryTile)};
-}
-
-// per-location totals: kept[loc] += keep counts, tested[loc] += tile counts
-__global__ void k_tile_totals(const QTile* tiles, const uint32_t* keep_counts, uint32_t ntiles, unsigned long long* kept,
-                              unsigned long long* tested) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= ntiles) return;
-    atomicAdd(&kept[tile_loc(tiles[i])], (unsigned long long)keep_counts[i]);
-    atomicAdd(&tested[tile_loc(tiles[i])], (unsigned long long)tiles[i].count);
-}
-
 // ---- LOD draw order applied at build time (lod_order.h): gather every node's points into their shuffled order ------------------
 struct LodArgs {
     const QNode* nodes;
@@ -506,7 +473,6 @@ struct BfsArgs {
     unsigned long long* bytes;   // sum of n * (3 bpc + 3) over the visited pairs
     int* overflow;
 };
-constexpr uint32_t kQueryTileBfs = 2048;
 __global__ void __launch_bounds__(256) k_bfs_level(const __grid_constant__ BfsArgs a) {
     const uint32_t n = min(*a.nin, a.cap);
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -522,7 +488,7 @@ __global__ void __launch_bounds__(256) k_bfs_level(const __grid_constant__ BfsAr
                 a.pairs[k] = make_uint2(g.kind == kLocCellUnion && rel == REL_IN ? (pr.x | kTileIn) : pr.x, pr.y);
             else
                 *a.overflow = 1;
-            atomicAdd(a.ntiles, (unsigned long long)((nd.n + kQueryTileBfs - 1) / kQueryTileBfs));
+            atomicAdd(a.ntiles, (unsigned long long)((nd.n + kQueryTile - 1) / kQueryTile));
             atomicAdd(&a.tested[pr.x], (unsigned long long)nd.n);
             atomicAdd(a.bytes, (unsigned long long)nd.n * (3ull * (unsigned long long)enc_bytes(nd.enc) + 3ull));
         }
