@@ -369,6 +369,21 @@ uint64_t tb_check_div(uint64_t n, uint64_t seed) {
     }
     return bad;
 }
+// The level table the build derives from a root cube (make_level_table, so PCV_CHECKED_FAST / PCV_NO_POW2 apply as in the
+// library): the division mode, the deepest level and the encoding of every level.  root_min may be NULL.
+void tb_level_table(double root_edge, double resolution, const double* root_min, int* fast, int* last_level, int8_t* enc) {
+    const LevelTable t = make_level_table(root_edge, resolution, root_min);
+    *fast = t.fast;
+    *last_level = t.last_level;
+    for (int L = 0; L < kMaxLevels; ++L) enc[L] = t.enc[L];
+}
+// div_known's Markstein sequence WITHOUT its range guard: what a kernel stores for a flagged numerator if the block did not
+// repeat the work with the IEEE operator
+double tb_div_unguarded(double a, double b, double y) {
+    const double q0 = a * y;
+    const double q1 = std::fma(std::fma(-q0, b, a), y, q0);
+    return std::fma(std::fma(-q1, b, a), y, q1);
+}
 // encode/decode fast == plain for random cubes at ECEF-like offsets, all encodings
 uint64_t tb_check_codec(uint64_t n, uint64_t seed) {
     uint64_t bad = 0, s = seed;

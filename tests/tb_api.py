@@ -27,8 +27,26 @@ def lib():
         L.tb_passes.argtypes = [C.c_void_p]
         L.tb_download.argtypes = [C.c_void_p] * 5
         L.tb_free.argtypes = [C.c_void_p]
+        L.tb_level_table.argtypes = [C.c_double, C.c_double, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p]
+        L.tb_div_unguarded.restype = C.c_double
+        L.tb_div_unguarded.argtypes = [C.c_double] * 3
         _lib = L
     return _lib
+
+
+def level_table(root_edge, resolution, root_min=None):
+    """make_level_table (csrc/build_host.hpp) as the build calls it: dict(fast, last_level, enc[41]).  PCV_CHECKED_FAST and
+    PCV_NO_POW2 in the environment apply as they do in the library."""
+    fast, last = C.c_int(), C.c_int()
+    enc = np.zeros(41, np.int8)
+    rm = (C.c_double * 3)(*[float(v) for v in root_min]) if root_min is not None else None
+    lib().tb_level_table(float(root_edge), float(resolution), rm, C.byref(fast), C.byref(last), enc.ctypes.data)
+    return dict(fast=fast.value, last_level=last.value, enc=[int(e) for e in enc])
+
+
+def div_unguarded(a, b, y):
+    """The reciprocal (Markstein) division of chain.h without its range guard."""
+    return lib().tb_div_unguarded(float(a), float(b), float(y))
 
 
 class TbTree:

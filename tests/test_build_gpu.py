@@ -33,6 +33,8 @@ def test_reference_scenario_100001(ctx):
 @pytest.mark.parametrize("n,maxpts,G,res", [(200000, 500, 3, 0.001), (200000, 500, 2, 0.001), (150000, 500, 1, 0.001),
                                              (50000, 50, 3, 1e-6), (300000, 1000, 3, 1e-9), (1000, 100000, 3, 0.001), (1, 100000, 3, 0.001)])
 def test_small_deep_trees(n, maxpts, G, res):
+    """G only seeds the cloud: levels_per_pass no longer changes the build (every pass resolves two levels, one when a single
+    level is left), so the G parametrisations are different clouds, not different pass schedules."""
     import point_cloud_viewer_b200 as pcv
 
     rng = np.random.default_rng(n + G)
@@ -119,28 +121,33 @@ def test_synth_host_device_identical(ctx):
 
 
 def test_degenerate_numerators_take_the_ieee_path(ctx):
-    """Zero, negative-zero, tiny (< 2^-500) and boundary coordinates: the reciprocal-division fast path flags them and the
-    block repeats its tile with the IEEE operator; results stay bit-identical to the oracle."""
+    """Zero, negative-zero, tiny (< 2^-500), subnormal and boundary coordinates in two boxes at the origin.  The unit box has
+    power-of-two edges (division mode 3): every quotient is an exact scaling and nothing is flagged.  The 0.75 box touches zero
+    with edges that are not powers of two (mode 1): the reciprocal division flags these numerators and the block repeats its
+    tile with the IEEE operator.  Both stay bit-identical to the oracle."""
     import point_cloud_viewer_b200 as pcv
+    from tb_api import level_table
 
     rng = np.random.default_rng(17)
     n = 60000
-    P = rng.random((n, 3))
-    P[:5000] = 0.0
-    P[5000:6000, 0] = -0.0
-    P[6000:7000, 1] = 1e-200
-    P[7000:8000, 2] = 5e-324
-    P[8000:9000] = 1.0  # on the max corner
-    P[9000:10000] = 0.5  # exactly on the centre planes (strict > decides)
-    x, y, z = [np.ascontiguousarray(P[:, i]) for i in range(3)]
-    rgb = rng.integers(0, 255, n * 3, dtype=np.uint8)
-    for maxpts, res in ((300, 1e-4), (2000, 1e-9)):
-        c = pcv.Context(0, max_points_per_node=maxpts)
-        tree = c.build_octree(x, y, z, rgb, res, (0, 0, 0), (1, 1, 1))
-        ref = O.build(x, y, z, rgb.reshape(-1, 3), res, (0, 0, 0), (1, 1, 1), max_points_per_node=maxpts)
-        compare_trees(ref, tree)
-        tree.free()
-        c.close()
+    for hi, mode in ((1.0, 3), (0.75, 1)):
+        P = rng.random((n, 3)) * hi
+        P[:5000] = 0.0
+        P[5000:6000, 0] = -0.0
+        P[6000:7000, 1] = 1e-200
+        P[7000:8000, 2] = 5e-324
+        P[8000:9000] = hi  # on the max corner
+        P[9000:10000] = hi / 2  # exactly on the centre planes (strict > decides)
+        x, y, z = [np.ascontiguousarray(P[:, i]) for i in range(3)]
+        rgb = rng.integers(0, 255, n * 3, dtype=np.uint8)
+        for maxpts, res in ((300, 1e-4), (2000, 1e-9)):
+            assert level_table(hi, res, (0.0, 0.0, 0.0))["fast"] == mode
+            c = pcv.Context(0, max_points_per_node=maxpts)
+            tree = c.build_octree(x, y, z, rgb, res, (0, 0, 0), (hi, hi, hi))
+            ref = O.build(x, y, z, rgb.reshape(-1, 3), res, (0, 0, 0), (hi, hi, hi), max_points_per_node=maxpts)
+            compare_trees(ref, tree)
+            tree.free()
+            c.close()
 
 
 def test_wild_inputs_with_unchecked_fast_path(ctx):
