@@ -235,14 +235,15 @@ struct PlaceArgs {
     uint32_t nleaves;
     uint32_t ntiles;
     uint64_t npoints, xyz_bytes;
-    uint32_t prefetch_tiles = 0;  // device backends: L2-prefetch the leaf tile this many blocks ahead (0 = off)
+    const LeafTile* tiles = nullptr;  // device backends: [ntiles] descriptor of every tile, written by the backend before the placement
     uint8_t* out_xyz;
     uint8_t* out_rgb;
     float* out_intensity;
     uint32_t* out_src;
 };
 
-// Tile descriptors are not materialised: a block finds its node by binary search over the per-node first-tile index.
+// A tile's node by binary search over the per-node first-tile index (the active-list lookup and the CPU test backend; the
+// CUDA placement materialises its tile descriptors instead, PlaceArgs::tiles).
 PCV_HD uint32_t upper_index(const uint32_t* begin, size_t stride_words, uint32_t n, uint32_t b) {
     uint32_t lo = 0, hi = n;  // largest i in [0, n) with begin[i] <= b
     while (hi - lo > 1) {
@@ -1096,8 +1097,8 @@ inline BuildResult assemble_top(Backend& be, double resolution, const double bmi
         cols[i] = (uint32_t)rgb[3 * i] | ((uint32_t)rgb[3 * i + 1] << 8) | ((uint32_t)rgb[3 * i + 2] << 16);
     }
     std::vector<void*> scratch;
-    auto up = [&](const void* h, size_t bytes) {
-        void* d = be.dmalloc(bytes ? bytes : 16);
+    auto up = [&](const void* h, size_t bytes, size_t slack = 0) {
+        void* d = be.dmalloc((bytes ? bytes : 16) + slack);
         scratch.push_back(d);
         if (bytes) be.h2d(d, h, bytes);
         return d;
@@ -1129,7 +1130,7 @@ inline BuildResult assemble_top(Backend& be, double resolution, const double bmi
     pl.wide = wide;
     pl.pts = PointsView{nullptr, nullptr, nullptr, 1, nullptr, intensity ? (const float*)up(intensity, (size_t)npoints * 4) : nullptr, npoints};
     pl.arena = up(recs.data(), recs.size());
-    pl.col_arena = (const uint32_t*)up(cols.data(), cols.size() * 4);
+    pl.col_arena = (const uint32_t*)up(cols.data(), cols.size() * 4, 64);  // + slack: the placement's bulk copies read whole 16-byte granules
     pl.fast = lv.fast;
     pl.d_nodes = (const DNode*)up(dn.data(), dn.size() * sizeof(DNode));
     pl.d_leaf_tile_begin = (const uint32_t*)up(leaf_tile_begin.data(), leaf_tile_begin.size() * 4);

@@ -96,18 +96,6 @@ __global__ void __launch_bounds__(256) k_bbox(PointsView p, double* __restrict__
 }
 
 // ------------------------------------------------------------------------------------------------
-// L2 prefetch of the tile the SM will work on one wave later
-// ------------------------------------------------------------------------------------------------
-// k_place streams leaf tiles whose addresses are known long before they are needed.  One thread asks the TMA unit to
-// pull the tile that is about one wave of resident blocks away into L2 (cp.async.bulk.prefetch.L2: no registers, no L1
-// lines, no completion to wait for), so that when that block runs its loads hit L2 instead of HBM.  The byte
-// range is shrunk to 16-byte alignment inside [p, p + bytes): nothing outside the caller's range is ever touched.
-__device__ __forceinline__ void l2_prefetch(const void* p, uint64_t bytes) {
-    const uintptr_t b = (reinterpret_cast<uintptr_t>(p) + 15) & ~(uintptr_t)15;
-    const uintptr_t e = (reinterpret_cast<uintptr_t>(p) + bytes) & ~(uintptr_t)15;
-    if (e > b) asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(b), "r"((uint32_t)(e - b)) : "memory");
-}
-// ------------------------------------------------------------------------------------------------
 // record load / store helpers
 // ------------------------------------------------------------------------------------------------
 template <bool WIDE>
@@ -121,23 +109,6 @@ struct RecT<true> {
     typedef RecW type;
 };
 
-template <bool WIDE>
-__device__ __forceinline__ void load_rec(const void* base, uint64_t i, uint64_t c[3], uint32_t& idx) {
-    if (WIDE) {
-        const ulonglong2* p = reinterpret_cast<const ulonglong2*>(base) + 2 * i;  // 32-byte record
-        const ulonglong2 v0 = __ldg(p), v1 = __ldg(p + 1);
-        c[0] = v0.x;
-        c[1] = v0.y;
-        c[2] = v1.x;
-        idx = (uint32_t)v1.y;
-    } else {
-        const uint4 v = __ldg(reinterpret_cast<const uint4*>(base) + i);  // 16-byte record
-        c[0] = v.x;
-        c[1] = v.y;
-        c[2] = v.z;
-        idx = v.w;
-    }
-}
 template <bool WIDE>
 __device__ __forceinline__ void store_rec(void* base, uint64_t i, const uint64_t c[3], uint32_t idx) {
     if (WIDE) {
@@ -1068,18 +1039,45 @@ __device__ __forceinline__ void place_store(const PlaceArgs& a, const DNode& nd,
     if (a.out_intensity) a.out_intensity[dp] = __ldg(a.pts.intensity + idx);
 }
 
+// A place tile staged in shared memory: its records, then its colours copied from the 16-byte granule that holds the first
+// one (scol[coff + i] is colour i, coff = arena_start & 3), the mbarrier of the copies and the tile's node (broadcast reads
+// instead of a node's worth of registers held through the whole tile).
+template <bool WIDE>
+struct PlaceSmem {
+    static constexpr size_t rec_bytes = WIDE ? 32 : 16;
+    static constexpr size_t off_col = (size_t)kPlaceTile * rec_bytes;
+    static constexpr size_t off_bar = off_col + ((size_t)kPlaceTile + 4) * 4;
+    static constexpr size_t off_node = off_bar + 16;
+    static constexpr size_t bytes = off_node + sizeof(DNode);
+    static_assert(off_col % 16 == 0 && off_bar % 16 == 0 && sizeof(DNode) % 4 == 0, "bulk copy destinations 16-byte aligned, the node copied in whole words");
+};
+static_assert(4 * (PlaceSmem<false>::bytes + 1024) <= 233472, "four narrow place blocks must fit one SM (228 KB, 1 KB reserved per block)");
+
+// tile -> descriptor (one block per leaf, threads over its tiles): a k_place block finds its tile with one load instead of a
+// binary search of dependent loads over the leaves' first tiles
+__global__ void k_place_tiles(const __grid_constant__ PlaceArgs a, LeafTile* __restrict__ tiles) {
+    const uint32_t l = blockIdx.x;
+    const uint32_t t0 = a.d_leaf_tile_begin[l], nt = a.d_leaf_tile_begin[l + 1] - t0;
+    const uint32_t node = a.d_leaf_node[l];
+    const uint64_t arena_off = a.d_nodes[node].arena_off, count = a.d_nodes[node].count;
+    for (uint32_t t = threadIdx.x; t < nt; t += blockDim.x) {
+        const uint64_t o = (uint64_t)t * kPlaceTile, rem = count - o;
+        tiles[t0 + t] = LeafTile{arena_off + o, o, node, (uint32_t)(rem < kPlaceTile ? rem : kPlaceTile)};
+    }
+}
+
 // The 7 of 8 points of a non-root node that stay: one same-cube rewrite (child_writer, generation.rs:234-238) with the
 // node's encoding hoisted out of the loop; dense lane mapping (stayer s <-> rank j = 8*(s/7) + s%7 + 1).
 template <bool WIDE, int ENC, int FAST>
-__device__ __forceinline__ unsigned place_stayers(const PlaceArgs& a, const LeafTile& lt, const DNode& nd) {
+__device__ __forceinline__ unsigned place_stayers(const PlaceArgs& a, const LeafTile& lt, const DNode& nd, const unsigned char* srec, const uint32_t* scol) {
     unsigned bad = 0;
     const uint32_t nst = lt.count - (lt.count + 7) / 8;  // tile starts at a multiple of 8
     for (uint32_t s = threadIdx.x; s < nst; s += blockDim.x) {
         const uint32_t i = 8 * (s / 7) + (s % 7) + 1;
         uint64_t c[3];
         uint32_t idx;
-        load_rec<WIDE>(a.arena, lt.arena_start + i, c, idx);
-        const uint32_t col = __ldg(a.col_arena + lt.arena_start + i);
+        smem_load_rec<WIDE>(srec, i, c, idx);
+        const uint32_t col = scol[i];
 #pragma unroll
         for (int k = 0; k < 3; ++k) c[k] = encode_axis<ENC, FAST>(decode_axis<ENC>(c[k], nd.m[k], nd.e), nd.m[k], nd.e, nd.ry, bad);
         if (!FAST || !bad) {
@@ -1092,83 +1090,98 @@ __device__ __forceinline__ unsigned place_stayers(const PlaceArgs& a, const Leaf
 
 // Points that move (every 8th by current rank, generation.rs:224-238): walk up re-encoding through every cube.
 template <bool WIDE>
-__device__ __forceinline__ void place_movers(const PlaceArgs& a, const LeafTile& lt, const DNode& leaf, bool all_points) {
+__device__ __forceinline__ void place_movers(const PlaceArgs& a, const LeafTile& lt, const DNode& leaf, bool all_points, const unsigned char* srec,
+                                             const uint32_t* scol) {
     const uint32_t step = all_points ? 1u : 8u;
     for (uint32_t i = threadIdx.x * step; i < lt.count; i += blockDim.x * step) {
         uint64_t c[3];
         uint32_t idx;
-        load_rec<WIDE>(a.arena, lt.arena_start + i, c, idx);
-        const uint32_t col = __ldg(a.col_arena + lt.arena_start + i);
+        smem_load_rec<WIDE>(srec, i, c, idx);
+        const uint32_t col = scol[i];
         uint64_t j = lt.j0 + i;
-        DNode nd = leaf;
-        while (nd.parent >= 0 && (j & 7) == 0) {
-            const DNode P = a.d_nodes[nd.parent];
+        const DNode* nd = &leaf;  // node fields are read where they are used: no node held in registers through the walk
+        while (nd->parent >= 0 && (j & 7) == 0) {
+            const DNode* P = a.d_nodes + nd->parent;
 #pragma unroll
             for (int k = 0; k < 3; ++k) {
                 if (a.fast) {
-                    const double q = decode1_fast(c[k], nd.m[k], nd.e, nd.enc);
-                    c[k] = encode1_fast(q, P.m[k], P.e, P.ry, P.enc);
+                    const double q = decode1_fast(c[k], nd->m[k], nd->e, nd->enc);
+                    c[k] = encode1_fast(q, P->m[k], P->e, P->ry, P->enc);
                 } else {
-                    const double q = decode1(c[k], nd.m[k], nd.e, nd.enc);
-                    c[k] = encode1(q, P.m[k], P.e, P.enc);
+                    const double q = decode1(c[k], nd->m[k], nd->e, nd->enc);
+                    c[k] = encode1(q, P->m[k], P->e, P->enc);
                 }
             }
-            j = nd.off_in_parent + (j >> 3);
+            j = nd->off_in_parent + (j >> 3);
             nd = P;
         }
         uint64_t slot = j;
-        if (nd.parent >= 0) {
+        if (nd->parent >= 0) {
 #pragma unroll
             for (int k = 0; k < 3; ++k) {
                 if (a.fast) {
-                    const double q = decode1_fast(c[k], nd.m[k], nd.e, nd.enc);
-                    c[k] = encode1_fast(q, nd.m[k], nd.e, nd.ry, nd.enc);
+                    const double q = decode1_fast(c[k], nd->m[k], nd->e, nd->enc);
+                    c[k] = encode1_fast(q, nd->m[k], nd->e, nd->ry, nd->enc);
                 } else {
-                    const double q = decode1(c[k], nd.m[k], nd.e, nd.enc);
-                    c[k] = encode1(q, nd.m[k], nd.e, nd.enc);
+                    const double q = decode1(c[k], nd->m[k], nd->e, nd->enc);
+                    c[k] = encode1(q, nd->m[k], nd->e, nd->enc);
                 }
             }
             slot = j - (j >> 3) - 1;
         }
-        place_store(a, nd, slot, c, col, idx);
+        place_store(a, *nd, slot, c, col, idx);
     }
 }
 
+// One block per place tile.  Thread 0 requests the whole tile - records and colours - with bulk copies into shared memory as
+// soon as the tile's descriptor is known; the node's descriptor is loaded while they are in flight, and no thread touches a
+// point before the copies have landed.  The records and colours stay staged for the FAST == 1 redo.
 template <bool WIDE>
 __global__ void __launch_bounds__(256) k_place(const __grid_constant__ PlaceArgs a) {
-    const LeafTile lt = leaf_tile_of(a, blockIdx.x);
-    const DNode leaf = a.d_nodes[lt.node];
-    if (threadIdx.x == 32 && a.prefetch_tiles) {  // leaf tiles are consecutive in the arena
-        const uint64_t first = lt.arena_start + (uint64_t)a.prefetch_tiles * kPlaceTile;
-        if (first < a.npoints) {
-            const uint64_t cnt = min((uint64_t)kPlaceTile, a.npoints - first), rb = WIDE ? 32 : 16;
-            l2_prefetch(reinterpret_cast<const unsigned char*>(a.arena) + first * rb, cnt * rb);
-            l2_prefetch(a.col_arena + first, cnt * 4);
-        }
+    constexpr size_t recsz = PlaceSmem<WIDE>::rec_bytes;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw + PlaceSmem<WIDE>::off_bar);
+    const LeafTile lt = a.tiles[blockIdx.x];
+    const uint32_t coff = (uint32_t)(lt.arena_start & 3);
+    if (threadIdx.x == 0) {
+        // records are 16 / 32 bytes, so the record range is 16-byte aligned; the colours are copied from the granule that
+        // holds the first one, rounded up to whole granules (every colour arena has slack past its end for that)
+        const uint32_t rec_bytes = lt.count * (uint32_t)recsz, col_bytes = ((coff + lt.count) * 4u + 15u) & ~15u;
+        mbar_init(bar, 1);
+        mbar_expect_tx(bar, rec_bytes + col_bytes);
+        tma_bulk_load(smem_raw, reinterpret_cast<const unsigned char*>(a.arena) + lt.arena_start * recsz, rec_bytes, bar);
+        tma_bulk_load(smem_raw + PlaceSmem<WIDE>::off_col, a.col_arena + (lt.arena_start - coff), col_bytes, bar);
     }
+    DNode* snode = reinterpret_cast<DNode*>(smem_raw + PlaceSmem<WIDE>::off_node);
+    if (threadIdx.x < sizeof(DNode) / 4) reinterpret_cast<uint32_t*>(snode)[threadIdx.x] = reinterpret_cast<const uint32_t*>(a.d_nodes + lt.node)[threadIdx.x];
+    const DNode& leaf = *snode;
+    const unsigned char* srec = smem_raw;
+    const uint32_t* scol = reinterpret_cast<const uint32_t*>(smem_raw + PlaceSmem<WIDE>::off_col) + coff;
+    __syncthreads();  // the barrier is initialised, the node is in shared memory
+    mbar_wait(bar, 0);
     // A tile whose start rank is not a multiple of 8 (top assembly: a collector's points start at arbitrary ranks), or
     // whose node ends the walk (root / collector), goes through the generic per-point path.
     const bool generic = leaf.parent < 0 || (lt.j0 & 7) != 0;
     if (generic) {
-        place_movers<WIDE>(a, lt, leaf, true);
+        place_movers<WIDE>(a, lt, leaf, true, srec, scol);
         return;
     }
     if (a.fast == 3) {
-        PCV_ENC_SWITCH(leaf.enc, place_stayers<WIDE, ENC, 3>(a, lt, leaf);)
+        PCV_ENC_SWITCH(leaf.enc, place_stayers<WIDE, ENC, 3>(a, lt, leaf, srec, scol);)
     } else if (a.fast) {
         unsigned bad = 0;
         if (a.fast == 2) {
-            PCV_ENC_SWITCH(leaf.enc, bad = place_stayers<WIDE, ENC, 2>(a, lt, leaf);)
+            PCV_ENC_SWITCH(leaf.enc, bad = place_stayers<WIDE, ENC, 2>(a, lt, leaf, srec, scol);)
         } else {
-            PCV_ENC_SWITCH(leaf.enc, bad = place_stayers<WIDE, ENC, 1>(a, lt, leaf);)
+            PCV_ENC_SWITCH(leaf.enc, bad = place_stayers<WIDE, ENC, 1>(a, lt, leaf, srec, scol);)
         }
         if (__syncthreads_or((int)bad)) {  // rare: redo the tile's stayers with the IEEE operator (idempotent stores)
-            PCV_ENC_SWITCH(leaf.enc, place_stayers<WIDE, ENC, 0>(a, lt, leaf);)
+            PCV_ENC_SWITCH(leaf.enc, place_stayers<WIDE, ENC, 0>(a, lt, leaf, srec, scol);)
         }
     } else {
-        PCV_ENC_SWITCH(leaf.enc, place_stayers<WIDE, ENC, 0>(a, lt, leaf);)
+        PCV_ENC_SWITCH(leaf.enc, place_stayers<WIDE, ENC, 0>(a, lt, leaf, srec, scol);)
     }
-    place_movers<WIDE>(a, lt, leaf, false);
+    place_movers<WIDE>(a, lt, leaf, false, srec, scol);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1366,20 +1379,18 @@ struct CudaBackend : Backend {
                         const void* fn = pass_kernel(w != 0, r != 0, f, e);
                         if (fn) cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(w ? PassSmem<true>::bytes : PassSmem<false>::bytes));
                     }
+        cudaFuncSetAttribute(k_place<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PlaceSmem<false>::bytes);
+        cudaFuncSetAttribute(k_place<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PlaceSmem<true>::bytes);
     }
-    // prefetch distance = blocks resident at once (SMs x blocks per SM); 0 disables (PCV_NO_PREFETCH=1 for experiments)
     int sms = 0;
-    bool no_prefetch = false;
     int sm_count() {
         if (!sms) {
             int dev = 0;
             cudaGetDevice(&dev);
             cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-            no_prefetch = std::getenv("PCV_NO_PREFETCH") != nullptr;
         }
         return sms;
     }
-    uint32_t resident(int blocks_per_sm) { return (sm_count(), no_prefetch) ? 0u : (uint32_t)(sms * blocks_per_sm); }
 
     void ingest(const IngestArgs& a) override {
         const uint32_t grid = std::min<uint32_t>(a.ntiles, (uint32_t)sm_count() * 32u);
@@ -1550,15 +1561,18 @@ struct CudaBackend : Backend {
     void place(const PlaceArgs& a_in) override {
         if (a_in.ntiles == 0) return;
         PlaceArgs a = a_in;
-        a.prefetch_tiles = resident(4);
+        LeafTile* tiles = (LeafTile*)dmalloc((size_t)a.ntiles * sizeof(LeafTile));
+        a.tiles = tiles;
         prof_begin(K_PLACE, a.npoints * ((a.wide ? sizeof(RecW) : sizeof(RecN)) + 3 + 3 + 4 + (a.out_intensity ? 8 : 0)) + a.xyz_bytes);
+        k_place_tiles<<<a.nleaves, 128, 0, stream>>>(a, tiles);
         if (a.wide)
-            k_place<true><<<a.ntiles, 256, 0, stream>>>(a);
+            k_place<true><<<a.ntiles, 256, PlaceSmem<true>::bytes, stream>>>(a);
         else
-            k_place<false><<<a.ntiles, 256, 0, stream>>>(a);
+            k_place<false><<<a.ntiles, 256, PlaceSmem<false>::bytes, stream>>>(a);
         prof_end();
-        ++launches;
+        launches += 2;
         PCV_CUDA_CHECK(cudaGetLastError());
+        dfree(tiles);
     }
 
     void bbox(const PointsView& p, double mn[3], double mx[3]) {
