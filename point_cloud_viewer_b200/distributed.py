@@ -125,9 +125,9 @@ class TorchComm:
         import torch
 
         s = torch.from_numpy(np.asarray(counts, np.int64)).to(self.device)
-        out = torch.empty((self.world, s.numel()), dtype=torch.int64, device=self.device)
+        out = torch.empty(self.world * s.numel(), dtype=torch.int64, device=self.device)  # flat: gloo takes no (world, n) output
         self.dist.all_gather_into_tensor(out, s)
-        return out.cpu().numpy()
+        return out.cpu().numpy().reshape(self.world, -1)
 
     def all_gather_bytes(self, buf, nbytes_max):
         """(world, nbytes_max) uint8 matrix: row r = rank r's byte buffer, zero padded (one tensor collective, no pickling)."""
@@ -136,9 +136,9 @@ class TorchComm:
         t = torch.zeros(nbytes_max, dtype=torch.uint8, device=self.device)
         if len(buf):
             t[: len(buf)] = torch.from_numpy(np.ascontiguousarray(buf, np.uint8)).to(self.device)
-        out = torch.empty((self.world, nbytes_max), dtype=torch.uint8, device=self.device)
+        out = torch.empty(self.world * nbytes_max, dtype=torch.uint8, device=self.device)
         self.dist.all_gather_into_tensor(out, t)
-        return out.cpu().numpy()
+        return out.cpu().numpy().reshape(self.world, nbytes_max)
 
     def barrier(self):
         if self.device.type == "cuda":
