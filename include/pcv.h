@@ -429,6 +429,25 @@ int pcv_s2_query_cell_unions_batch_device(const pcv_s2cloud* cloud, const pcv_ce
  * octree metas are rejected with the reference's messages). */
 int pcv_s2_write_dir(const pcv_s2cloud* cloud, const char* directory);
 int pcv_s2_load_dir(pcv_ctx* ctx, const char* directory, pcv_s2cloud** out);
+/* build_xray_quadtree over an S2 cloud (xray/src/build_quadtree.rs with S2 locations), in bounded device memory like
+ * pcv_xray_quadtree_bounded[_write_dir]: the same post-order delivery, cancellation, <id>.png + meta[<digits>].pb output and
+ * pcv_xray_bounded_info.  The quadtree's frame, rect and levels come from the cloud's box (pcv_s2_info: the exact min and max
+ * of the stored positions, S2Splitter::get_meta's box), a leaf's location is the Aabb (or, with query_from_global, the Obb) the
+ * octree driver builds for it, and a leaf's points are every stored point p (the stored doubles) with loc.contains(p) and
+ * lo <= (double)intensity <= hi for every filter interval: xray_from_points over FilteredIterator without the reference's
+ * rectangle pre-selection, so a superset of the reference's points as for the S2 location queries.  A leaf exists iff that set
+ * is not empty.  XRay tiles are exact; Colored, ColoredWithIntensity and ColoredWithHeightStddev (Binning = None) accumulate
+ * like pcv_xray_tile_attr.  Binned strategies (bin_size != 0) are PCV_ERR_UNSUPPORTED; filters on a cloud without intensity
+ * and Colored on a cloud without colour are PCV_ERR_INVALID.  max_device_bytes (0: most of the free memory) bounds what the
+ * call allocates besides the cloud's arrays and its location tables; info.leaf_points counts the points every binning pass
+ * reads.  A block's points are read once to count every leaf's keys and once per key batch to place them (the attribute
+ * strategies: once per batch of leaves whose per-pixel sums fit the budget). */
+int pcv_s2_xray_quadtree(const pcv_s2cloud* cloud, const pcv_xray_quadtree_params* params, const pcv_interval* filters, uint32_t nfilt,
+                         uint64_t max_device_bytes, pcv_xray_tile_fn on_tile, void* user, pcv_xray_quadtree_info* info_out,
+                         pcv_xray_bounded_info* bounded_info_out);
+int pcv_s2_xray_quadtree_write_dir(const pcv_s2cloud* cloud, const pcv_xray_quadtree_params* params, const pcv_interval* filters, uint32_t nfilt,
+                                   uint64_t max_device_bytes, const char* directory, pcv_xray_quadtree_info* info_out,
+                                   pcv_xray_bounded_info* bounded_info_out);
 /* CellUnion::contains for arbitrary points: mask_out[i] = union.contains_cellid(CellID::from_point(p_i)). */
 int pcv_s2_union_contains(pcv_ctx* ctx, const pcv_points* host_points, const uint64_t* union_ids, uint32_t n_union, uint8_t* mask_out);
 

@@ -590,6 +590,23 @@ class S2Cells {
         tested.assign(unions.size(), 0);
         check(pcv_s2_query_cell_unions_batch_device(s_, raw.data(), (uint32_t)raw.size(), nullptr, 0, counts.data(), tested.data()));
     }
+    // build_xray_quadtree (xray/src/build_quadtree.rs) over the cloud, with the leaf queries' filter intervals: every tile through
+    // `on_tile` in post-order, as Octree::build_xray_quadtree delivers it.  `max_device_bytes` bounds the call's device memory.
+    template <class F>
+    pcv_xray_quadtree_info xray_quadtree(const pcv_xray_quadtree_params& params, const std::vector<ClosedInterval>& filter_intervals, F&& on_tile,
+                                         uint64_t max_device_bytes = 0, pcv_xray_bounded_info* bounded_info = nullptr) const {
+        struct Thunk {
+            F* f;
+            static int call(void* user, uint8_t level, uint64_t index, const uint8_t* rgba, uint32_t tile_px) {
+                (*static_cast<Thunk*>(user)->f)(level, index, rgba, tile_px);
+                return 0;
+            }
+        } th{&on_tile};
+        const std::vector<pcv_interval> f = detail::raw_intervals(filter_intervals);
+        pcv_xray_quadtree_info info{};
+        check(pcv_s2_xray_quadtree(s_, &params, f.data(), (uint32_t)f.size(), max_device_bytes, &Thunk::call, &th, &info, bounded_info));
+        return info;
+    }
     void write_to_directory(const std::string& dir) const { check(pcv_s2_write_dir(s_, dir.c_str())); }
     pcv_s2cloud* raw() const { return s_; }
 

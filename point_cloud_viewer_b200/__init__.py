@@ -881,6 +881,36 @@ class S2Cloud:
         N.check(N.lib().pcv_last_query_stats(self.ctx.h, C.byref(st)))
         return {k: getattr(st, k) for k, _ in N.QueryStats._fields_}
 
+    def xray_quadtree(self, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0, query_from_global=None,
+                      background=(255, 255, 255, 255), root=(0, 0), on_tile=None, keep_tiles=True, filter_intervals=(), max_device_bytes=0):
+        """Octree.xray_quadtree over the cloud (pcv_s2_xray_quadtree): the quadtree over the cloud's box, every leaf made of the
+        stored points its location contains that pass `filter_intervals` ((lo, hi) pairs on the intensity, closed).  Returns
+        (info dict, {(level, index): RGBA array}); `on_tile` and `max_device_bytes` as in Octree.xray_quadtree."""
+        pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
+        f = np.ascontiguousarray(np.asarray(filter_intervals, np.float64).reshape(-1))
+        tiles = {}
+
+        def cb(_user, level, index, ptr, tpx):
+            img = np.ctypeslib.as_array(ptr, shape=(tpx, tpx, 4))
+            if keep_tiles:
+                tiles[(int(level), int(index))] = img.copy()
+            return 1 if (on_tile is not None and on_tile(int(level), int(index), img)) else 0
+
+        info, binfo = N.XrayQuadtreeInfo(), N.XrayBoundedInfo()
+        N.check(N.lib().pcv_s2_xray_quadtree(self.h, C.byref(pr), _p(f) if len(f) else None, len(f) // 2, int(max_device_bytes), N.XRAY_TILE_FN(cb), None,
+                                             C.byref(info), C.byref(binfo)))
+        return _xray_info(info, binfo), tiles
+
+    def xray_quadtree_write_dir(self, directory, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0, query_from_global=None,
+                                background=(255, 255, 255, 255), root=(0, 0), filter_intervals=(), max_device_bytes=0):
+        """xray_quadtree with the reference's outputs: <directory>/<node id>.png + the quadtree's meta file."""
+        pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
+        f = np.ascontiguousarray(np.asarray(filter_intervals, np.float64).reshape(-1))
+        info, binfo = N.XrayQuadtreeInfo(), N.XrayBoundedInfo()
+        N.check(N.lib().pcv_s2_xray_quadtree_write_dir(self.h, C.byref(pr), _p(f) if len(f) else None, len(f) // 2, int(max_device_bytes),
+                                                       os.fsencode(str(directory)), C.byref(info), C.byref(binfo)))
+        return _xray_info(info, binfo)
+
 
 def s2_token(cell_id):
     """CellID::to_token: the per-cell file stem of the reference's S2 directory layout."""

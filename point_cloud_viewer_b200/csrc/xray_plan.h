@@ -3,7 +3,9 @@
 //   xray_key_batches:     consecutive leaves of a block grouped so that their possible keys fit the key buffer
 //   xray_levels_to_close: the post-order bookkeeping - which ancestors are complete when the walk moves on to the next subtree
 //   xray_post_order:      every node of a subtree with the given leaves, each after all of its children
+//   s2_xray_plan:         the S2 cloud's leaf producer (s2_xray.inl): block depth, key capacity and attribute batch size
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <utility>
 #include <vector>
@@ -73,6 +75,33 @@ inline std::vector<std::pair<int, uint64_t>> xray_post_order(const std::vector<u
         for (int up = 1; up <= k; ++up) out.emplace_back(up, leaves[i] >> (2 * up));
     }
     return out;
+}
+
+// ---- the leaf producer of an S2 cloud (s2_xray.inl) --------------------------------------------------------------------------
+// What it holds besides the run's fixed set (taps, mosaic, grey table, one attribute slice): the pruning pass's work list of
+// every cell and the block's cell tiles, at most every tile again (16 B per tile each), the cell selection of one location (an
+// 8 B pair per cell, 64 B of counters) and the filter intervals (16 B each).
+inline uint64_t s2_xray_fixed_bytes(uint64_t ncells, uint64_t ntiles, uint32_t nfilt) { return 32 * ntiles + 8 * ncells + 16ull * nfilt + 4096; }
+
+struct S2XrayPlan {
+    int g = -1;                // block depth (xray_block_depth); -1: not even one leaf fits
+    uint64_t key_cap = 0;      // XRay: keys of one batch
+    uint64_t attr_leaves = 0;  // attribute strategies: leaves whose slices one accumulation pass holds
+    uint64_t descent_chunk = 0;  // candidates per pruning pass (8 B index + 4 B flag each; no block is held meanwhile)
+};
+// `fixed` holds one attribute slice (`slice_bytes`, 0 for XRay); `leaf_bytes` everything a candidate leaf holds (image,
+// XrayArgs, seen flag, and 4 B of count plus 4 B of offset per bin).  After the block's images, what the budget leaves goes to
+// 4-byte keys or to further slices.  The pruning descent runs before any block and may use all of what `fixed` leaves.
+inline S2XrayPlan s2_xray_plan(uint64_t budget, uint64_t fixed, int depth, int max_g, uint64_t leaf_bytes, uint64_t tile_bytes, uint64_t slice_bytes) {
+    S2XrayPlan p;
+    p.descent_chunk = budget > fixed ? std::max<uint64_t>(1, (budget - fixed) / 16) : 1;
+    p.g = xray_block_depth(budget, fixed, depth, max_g, leaf_bytes, tile_bytes);
+    if (p.g < 0) return p;
+    const uint64_t used = fixed + xray_block_bytes(p.g, depth - p.g, leaf_bytes, tile_bytes);
+    const uint64_t rest = budget > used ? budget - used : 0;
+    p.key_cap = std::min<uint64_t>(rest / 4, 0xFFFFFFFEull);
+    p.attr_leaves = slice_bytes ? 1 + rest / slice_bytes : 0;
+    return p;
 }
 
 }  // namespace pcv
