@@ -182,27 +182,15 @@ class Context:
         and keywords.  `max_device_bytes` bounds everything the call allocates (0: most of the free memory); the info dict also
         holds the pcv_xray_dir_info fields."""
         pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
-        tiles = {}
-
-        def cb(_user, level, index, ptr, tpx):
-            img = np.ctypeslib.as_array(ptr, shape=(tpx, tpx, 4))
-            if keep_tiles:
-                tiles[(int(level), int(index))] = img.copy()
-            return 1 if (on_tile is not None and on_tile(int(level), int(index), img)) else 0
-
-        info, binfo, dinfo = N.XrayQuadtreeInfo(), N.XrayBoundedInfo(), N.XrayDirInfo()
-        N.check(N.lib().pcv_xray_quadtree_from_dir(self.h, os.fsencode(str(octree_dir)), C.byref(pr), int(max_device_bytes), N.XRAY_TILE_FN(cb), None,
-                                                   C.byref(info), C.byref(binfo), C.byref(dinfo)))
-        return _xray_info(info, binfo, dinfo), tiles
+        return _xray_call(N.lib().pcv_xray_quadtree_from_dir, (self.h, os.fsencode(str(octree_dir)), C.byref(pr), int(max_device_bytes)), True, True, on_tile,
+                          keep_tiles)
 
     def xray_quadtree_from_dir_write_dir(self, octree_dir, out_dir, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0,
                                          query_from_global=None, background=(255, 255, 255, 255), root=(0, 0), max_device_bytes=0):
         """xray_quadtree_from_dir with the reference's outputs: <out_dir>/<node id>.png + the quadtree's meta file."""
         pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
-        info, binfo, dinfo = N.XrayQuadtreeInfo(), N.XrayBoundedInfo(), N.XrayDirInfo()
-        N.check(N.lib().pcv_xray_quadtree_from_dir_write_dir(self.h, os.fsencode(str(octree_dir)), C.byref(pr), int(max_device_bytes),
-                                                             os.fsencode(str(out_dir)), C.byref(info), C.byref(binfo), C.byref(dinfo)))
-        return _xray_info(info, binfo, dinfo)
+        return _xray_call(N.lib().pcv_xray_quadtree_from_dir_write_dir,
+                          (self.h, os.fsencode(str(octree_dir)), C.byref(pr), int(max_device_bytes), os.fsencode(str(out_dir))), True)
 
     def open_dir(self, directory, max_device_bytes=0):
         """An OctreeDir over the octree in `directory`: queries read only the nodes they select (0: most of the free memory)."""
@@ -637,26 +625,13 @@ class Octree:
         true value to cancel).  `max_device_bytes` bounds the driver's device memory (0: most of the free memory); the info
         dict holds the pcv_xray_quadtree_info and pcv_xray_bounded_info fields."""
         pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
-        tiles = {}
-
-        def cb(_user, level, index, ptr, tpx):
-            img = np.ctypeslib.as_array(ptr, shape=(tpx, tpx, 4))
-            if keep_tiles:
-                tiles[(int(level), int(index))] = img.copy()
-            return 1 if (on_tile is not None and on_tile(int(level), int(index), img)) else 0
-
-        info, binfo = N.XrayQuadtreeInfo(), N.XrayBoundedInfo()
-        N.check(N.lib().pcv_xray_quadtree_bounded(self.h, C.byref(pr), int(max_device_bytes), N.XRAY_TILE_FN(cb), None, C.byref(info), C.byref(binfo)))
-        return _xray_info(info, binfo), tiles
+        return _xray_call(N.lib().pcv_xray_quadtree_bounded, (self.h, C.byref(pr), int(max_device_bytes)), False, True, on_tile, keep_tiles)
 
     def xray_quadtree_write_dir(self, directory, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0, query_from_global=None,
                                 background=(255, 255, 255, 255), root=(0, 0), max_device_bytes=0):
         """build_xray_quadtree with the reference's outputs: <directory>/<node id>.png + the quadtree's meta file."""
         pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
-        info, binfo = N.XrayQuadtreeInfo(), N.XrayBoundedInfo()
-        N.check(N.lib().pcv_xray_quadtree_bounded_write_dir(self.h, C.byref(pr), int(max_device_bytes), os.fsencode(str(directory)), C.byref(info),
-                                                            C.byref(binfo)))
-        return _xray_info(info, binfo)
+        return _xray_call(N.lib().pcv_xray_quadtree_bounded_write_dir, (self.h, C.byref(pr), int(max_device_bytes), os.fsencode(str(directory))), False)
 
 
 def _loc_arg(loc):
@@ -888,28 +863,16 @@ class S2Cloud:
         (info dict, {(level, index): RGBA array}); `on_tile` and `max_device_bytes` as in Octree.xray_quadtree."""
         pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
         f = np.ascontiguousarray(np.asarray(filter_intervals, np.float64).reshape(-1))
-        tiles = {}
-
-        def cb(_user, level, index, ptr, tpx):
-            img = np.ctypeslib.as_array(ptr, shape=(tpx, tpx, 4))
-            if keep_tiles:
-                tiles[(int(level), int(index))] = img.copy()
-            return 1 if (on_tile is not None and on_tile(int(level), int(index), img)) else 0
-
-        info, binfo = N.XrayQuadtreeInfo(), N.XrayBoundedInfo()
-        N.check(N.lib().pcv_s2_xray_quadtree(self.h, C.byref(pr), _p(f) if len(f) else None, len(f) // 2, int(max_device_bytes), N.XRAY_TILE_FN(cb), None,
-                                             C.byref(info), C.byref(binfo)))
-        return _xray_info(info, binfo), tiles
+        return _xray_call(N.lib().pcv_s2_xray_quadtree, (self.h, C.byref(pr), _p(f) if len(f) else None, len(f) // 2, int(max_device_bytes)), False, True, on_tile,
+                          keep_tiles)
 
     def xray_quadtree_write_dir(self, directory, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0, query_from_global=None,
                                 background=(255, 255, 255, 255), root=(0, 0), filter_intervals=(), max_device_bytes=0):
         """xray_quadtree with the reference's outputs: <directory>/<node id>.png + the quadtree's meta file."""
         pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
         f = np.ascontiguousarray(np.asarray(filter_intervals, np.float64).reshape(-1))
-        info, binfo = N.XrayQuadtreeInfo(), N.XrayBoundedInfo()
-        N.check(N.lib().pcv_s2_xray_quadtree_write_dir(self.h, C.byref(pr), _p(f) if len(f) else None, len(f) // 2, int(max_device_bytes),
-                                                       os.fsencode(str(directory)), C.byref(info), C.byref(binfo)))
-        return _xray_info(info, binfo)
+        return _xray_call(N.lib().pcv_s2_xray_quadtree_write_dir,
+                          (self.h, C.byref(pr), _p(f) if len(f) else None, len(f) // 2, int(max_device_bytes), os.fsencode(str(directory))), False)
 
 
 def s2_token(cell_id):
@@ -942,12 +905,25 @@ def _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_siz
     return pr
 
 
-def _xray_info(info, binfo, dinfo=None):
-    out = {k: getattr(info, k) for k, _ in N.XrayQuadtreeInfo._fields_}
-    out.update({k: getattr(binfo, k) for k, _ in N.XrayBoundedInfo._fields_})
-    if dinfo is not None:
-        out.update({k: getattr(dinfo, k) for k, _ in N.XrayDirInfo._fields_})
-    return out
+def _xray_call(fn, args, dir_info, with_tiles=False, on_tile=None, keep_tiles=True):
+    """One X-ray quadtree entry: fn(*args, [tile callback, None,] info, bounded info[, dir info]).  Returns the info dict, or
+    `with_tiles` the entry takes the tile callback and the result is (info dict, {(level, index): RGBA array}): every tile goes
+    to on_tile(level, index, rgba), whose true value cancels, and is kept if keep_tiles."""
+    infos = [N.XrayQuadtreeInfo(), N.XrayBoundedInfo()] + ([N.XrayDirInfo()] if dir_info else [])
+    tiles = {}
+
+    def cb(_user, level, index, ptr, tpx):
+        img = np.ctypeslib.as_array(ptr, shape=(tpx, tpx, 4))
+        if keep_tiles:
+            tiles[(int(level), int(index))] = img.copy()
+        return 1 if (on_tile is not None and on_tile(int(level), int(index), img)) else 0
+
+    callback = (N.XRAY_TILE_FN(cb), None) if with_tiles else ()
+    N.check(fn(*args, *callback, *[C.byref(i) for i in infos]))
+    out = {}
+    for i in infos:
+        out.update({k: getattr(i, k) for k, _ in i._fields_})
+    return (out, tiles) if with_tiles else out
 
 
 def xray_assign_background(ctx, rgba, background):

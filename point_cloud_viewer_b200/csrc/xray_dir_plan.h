@@ -6,7 +6,6 @@
 //   xray_window:            the nodes a block of leaves can meet: descend from the octree root while the SAT test is not Out
 //   xray_window_size:       what one window takes in device memory (arrays, query tables, the attribute pass flags)
 //   xray_block_location:    a block's location, widened by the pruning margin
-//   xray_select_share:      the budget's share for the node selection (the bounded driver's split)
 //   xray_dir_block_depth:   the block depth from the budget, the images and the largest window of the occupied blocks
 #pragma once
 #include <algorithm>
@@ -158,20 +157,6 @@ inline pcv_location xray_block_location(const QuadRect& rect, int B, uint64_t bi
     return xray_location(tmin, tmax, qfg);
 }
 
-// The bounded driver's split of what the budget leaves after `fixed`: an eighth for the node selection (frontier capacity
-// `sel_cap` pairs and `max_loc` locations per selection), the rest for the block's images and a key batch.
-struct XraySelectShare {
-    uint64_t sel_bytes = 0, max_loc = 0;
-    uint32_t sel_cap = 0;
-};
-inline XraySelectShare xray_select_share(uint64_t budget, uint64_t fixed, uint64_t per_loc) {
-    XraySelectShare s;
-    s.sel_bytes = budget > fixed ? (budget - fixed) / 8 : 0;
-    s.sel_cap = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(s.sel_bytes / 2 / 40, 64), 48ull << 20);
-    s.max_loc = std::max<uint64_t>(1, s.sel_bytes / 2 / per_loc);
-    return s;
-}
-
 // Block depth g of the directory driver: the largest g <= g_max for which the block images, the node selection and the
 // largest window over the occupied blocks at level deepest - g (`window_max(g)`, UINT64_MAX: a window too large to hold) fit
 // the budget besides `fixed`.  A smaller g means a deeper block level and smaller windows.  -1: not even g = 0 fits.
@@ -179,9 +164,7 @@ inline int xray_dir_block_depth(uint64_t budget, uint64_t fixed, int depth, int 
                                 const std::function<uint64_t(int)>& window_max) {
     for (int g = g_max; g >= 0; --g) {
         const uint64_t w = window_max(g);
-        if (w == UINT64_MAX || fixed + w >= budget) continue;
-        const XraySelectShare s = xray_select_share(budget, fixed + w, per_loc);
-        if (xray_block_depth(budget, fixed + w + s.sel_bytes + 40ull * s.sel_cap, depth, g, leaf_bytes, tile_bytes) >= g) return g;
+        if (w != UINT64_MAX && xray_octree_plan(budget, fixed, w, depth, g, per_loc, leaf_bytes, tile_bytes).g == g) return g;
     }
     return -1;
 }

@@ -3,6 +3,7 @@
 //   xray_key_batches:     consecutive leaves of a block grouped so that their possible keys fit the key buffer
 //   xray_levels_to_close: the post-order bookkeeping - which ancestors are complete when the walk moves on to the next subtree
 //   xray_post_order:      every node of a subtree with the given leaves, each after all of its children
+//   xray_octree_plan:     the octree sources' plan: block depth, node selection and key capacity
 //   s2_xray_plan:         the S2 cloud's leaf producer (s2_xray.inl): block depth, key capacity and attribute batch size
 #pragma once
 #include <algorithm>
@@ -77,24 +78,48 @@ inline std::vector<std::pair<int, uint64_t>> xray_post_order(const std::vector<u
     return out;
 }
 
+// What the driver runs with, from the budget: the block depth, the node selection's frontier capacity and locations per
+// selection (octree sources) or candidates per pruning pass (S2), and what a block's leaves may hold besides their images.
+struct XrayPlan {
+    int g = -1;                // block depth (xray_block_depth); -1: not even one leaf fits
+    uint32_t sel_cap = 0;      // octree sources: frontier pairs of one node selection
+    uint64_t max_loc = 0;      // locations per node selection, or per pruning pass
+    uint64_t key_cap = 0;      // XRay: keys of one batch
+    uint64_t attr_leaves = 0;  // S2 attribute strategies: leaves whose slices one accumulation pass holds
+};
+
+// The plan of an octree source: `fixed` bytes for the whole run and `window` bytes of points (0 for a resident octree; the
+// largest window of the blocks for an octree directory).  An eighth of what they leave goes to the node selection (half to
+// its frontier, `sel_cap` pairs and 40 B more per pair, half to `max_loc` locations of `per_loc` bytes); g is the largest
+// block depth <= max_g whose images fit besides; what remains after the block's images holds the keys of a batch, 4 bytes per
+// key and its share of the work tiles.
+inline XrayPlan xray_octree_plan(uint64_t budget, uint64_t fixed, uint64_t window, int depth, int max_g, uint64_t per_loc, uint64_t leaf_bytes,
+                                 uint64_t tile_bytes) {
+    XrayPlan p;
+    const uint64_t sel_bytes = budget > fixed + window ? (budget - fixed - window) / 8 : 0;
+    p.sel_cap = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(sel_bytes / 2 / 40, 64), 48ull << 20);
+    p.max_loc = std::max<uint64_t>(1, sel_bytes / 2 / per_loc);
+    const uint64_t held = fixed + window + sel_bytes + 40ull * p.sel_cap;
+    p.g = xray_block_depth(budget, held, depth, max_g, leaf_bytes, tile_bytes);
+    if (p.g < 0) return p;
+    const uint64_t used = held + xray_block_bytes(p.g, depth - p.g, leaf_bytes, tile_bytes);
+    p.key_cap = budget > used ? std::min<uint64_t>((budget - used) / 5, 0xFFFFFFFEull) : 0;
+    return p;
+}
+
 // ---- the leaf producer of an S2 cloud (s2_xray.inl) --------------------------------------------------------------------------
 // What it holds besides the run's fixed set (taps, mosaic, grey table, one attribute slice): the pruning pass's work list of
 // every cell and the block's cell tiles, at most every tile again (16 B per tile each), the cell selection of one location (an
 // 8 B pair per cell, 64 B of counters) and the filter intervals (16 B each).
 inline uint64_t s2_xray_fixed_bytes(uint64_t ncells, uint64_t ntiles, uint32_t nfilt) { return 32 * ntiles + 8 * ncells + 16ull * nfilt + 4096; }
 
-struct S2XrayPlan {
-    int g = -1;                // block depth (xray_block_depth); -1: not even one leaf fits
-    uint64_t key_cap = 0;      // XRay: keys of one batch
-    uint64_t attr_leaves = 0;  // attribute strategies: leaves whose slices one accumulation pass holds
-    uint64_t descent_chunk = 0;  // candidates per pruning pass (8 B index + 4 B flag each; no block is held meanwhile)
-};
 // `fixed` holds one attribute slice (`slice_bytes`, 0 for XRay); `leaf_bytes` everything a candidate leaf holds (image,
 // XrayArgs, seen flag, and 4 B of count plus 4 B of offset per bin).  After the block's images, what the budget leaves goes to
-// 4-byte keys or to further slices.  The pruning descent runs before any block and may use all of what `fixed` leaves.
-inline S2XrayPlan s2_xray_plan(uint64_t budget, uint64_t fixed, int depth, int max_g, uint64_t leaf_bytes, uint64_t tile_bytes, uint64_t slice_bytes) {
-    S2XrayPlan p;
-    p.descent_chunk = budget > fixed ? std::max<uint64_t>(1, (budget - fixed) / 16) : 1;
+// 4-byte keys or to further slices.  The pruning descent runs before any block and may use all of what `fixed` leaves, 16 B
+// per candidate (8 B index + 4 B flag; no block is held meanwhile).
+inline XrayPlan s2_xray_plan(uint64_t budget, uint64_t fixed, int depth, int max_g, uint64_t leaf_bytes, uint64_t tile_bytes, uint64_t slice_bytes) {
+    XrayPlan p;
+    p.max_loc = budget > fixed ? std::max<uint64_t>(1, (budget - fixed) / 16) : 1;
     p.g = xray_block_depth(budget, fixed, depth, max_g, leaf_bytes, tile_bytes);
     if (p.g < 0) return p;
     const uint64_t used = fixed + xray_block_bytes(p.g, depth - p.g, leaf_bytes, tile_bytes);

@@ -19,8 +19,8 @@ int main() {
     if (what == "plan") {
         unsigned long long budget, fixed, leaf, tile, slice; int depth, maxg;
         std::cin >> budget >> fixed >> depth >> maxg >> leaf >> tile >> slice;
-        const pcv::S2XrayPlan p = pcv::s2_xray_plan(budget, fixed, depth, maxg, leaf, tile, slice);
-        std::cout << p.g << " " << p.key_cap << " " << p.attr_leaves << " " << p.descent_chunk << "\n";
+        const pcv::XrayPlan p = pcv::s2_xray_plan(budget, fixed, depth, maxg, leaf, tile, slice);
+        std::cout << p.g << " " << p.key_cap << " " << p.attr_leaves << " " << p.max_loc << " " << p.sel_cap << "\n";
     } else if (what == "fixed") {
         unsigned long long nc, nt; unsigned nf;
         std::cin >> nc >> nt >> nf;
@@ -55,10 +55,10 @@ def plan_py(budget, fixed, depth, maxg, leaf, tile, slice_bytes):
     chunk = max(1, (budget - fixed) // 16) if budget > fixed else 1
     g = depth_py(budget, fixed, depth, maxg, leaf, tile)
     if g < 0:
-        return -1, 0, 0, chunk
+        return -1, 0, 0, chunk, 0
     used = fixed + block_bytes(g, depth - g, leaf, tile)
     rest = max(budget - used, 0)
-    return g, min(rest // 4, 0xFFFFFFFE), (1 + rest // slice_bytes) if slice_bytes else 0, chunk
+    return g, min(rest // 4, 0xFFFFFFFE), (1 + rest // slice_bytes) if slice_bytes else 0, chunk, 0
 
 
 def test_plan_matches_restatement(plan):

@@ -1,5 +1,6 @@
 """Bounded X-ray quadtree: the planner (csrc/xray_plan.h, compiled here with g++) against a Python restatement - block depth
-from the budget, key-batch splits, the post-order of a sparse leaf set - and the pcv_xray_bounded_info layout.  No GPU."""
+from the budget, the octree sources' plan, key-batch splits, the post-order of a sparse leaf set - and the
+pcv_xray_bounded_info layout.  No GPU."""
 import ctypes as C
 import os
 import subprocess
@@ -19,6 +20,11 @@ int main() {
         unsigned long long budget, fixed, leaf, tile; int depth, maxg;
         std::cin >> budget >> fixed >> depth >> maxg >> leaf >> tile;
         std::cout << pcv::xray_block_depth(budget, fixed, depth, maxg, leaf, tile) << "\n";
+    } else if (what == "octree") {
+        unsigned long long budget, fixed, window, per_loc, leaf, tile; int depth, maxg;
+        std::cin >> budget >> fixed >> window >> depth >> maxg >> per_loc >> leaf >> tile;
+        const pcv::XrayPlan p = pcv::xray_octree_plan(budget, fixed, window, depth, maxg, per_loc, leaf, tile);
+        std::cout << p.g << " " << p.sel_cap << " " << p.max_loc << " " << p.key_cap << " " << p.attr_leaves << "\n";
     } else if (what == "batches") {
         size_t n; unsigned long long cap;
         std::cin >> n >> cap;
@@ -65,6 +71,20 @@ def depth_py(budget, fixed, depth, maxg, leaf, tile):
     return g
 
 
+def octree_plan_py(budget, fixed, window, depth, maxg, per_loc, leaf, tile):
+    """(g, sel_cap, max_loc, key_cap, attr_leaves): an eighth of what fixed + window leave for the node selection, the block
+    depth besides it, and the rest after the block's images for keys of 5 bytes each."""
+    sel = (budget - fixed - window) // 8 if budget > fixed + window else 0
+    cap = min(max(sel // 2 // 40, 64), 48 << 20)
+    loc = max(1, sel // 2 // per_loc)
+    held = fixed + window + sel + 40 * cap
+    g = depth_py(budget, held, depth, maxg, leaf, tile)
+    if g < 0:
+        return g, cap, loc, 0, 0
+    used = held + block_bytes(g, depth - g, leaf, tile)
+    return g, cap, loc, min((budget - used) // 5, 0xFFFFFFFE) if budget > used else 0, 0
+
+
 def batches_py(keys, cap):
     starts, run = [], 0
     for i, k in enumerate(keys):
@@ -105,6 +125,25 @@ def test_block_depth(plan):
                 for fixed in (0, 2 * tile + 5000):
                     got = int(plan("depth %d %d %d 10 %d %d\n" % (budget, fixed, depth, leaf, tile))[0])
                     assert got == depth_py(budget, fixed, depth, 10, leaf, tile), (tile, depth, budget, fixed)
+
+
+def test_octree_plan(plan):
+    rng = np.random.default_rng(5)
+    for _ in range(300):
+        T = int(rng.choice([16, 64, 256, 1024]))
+        tile = T * T * 4
+        leaf = tile + 8 * (-(-T // 32) ** 2 + 1) + int(rng.integers(600, 1200))
+        fixed = 2 * tile + int(rng.integers(0, 1 << 20))
+        window = 0 if rng.random() < 0.5 else int(rng.integers(0, 1 << 28))
+        budget = int(rng.choice([fixed, fixed + window, int(np.exp(rng.uniform(np.log(tile), np.log(80 * 2 ** 30))))]))
+        depth, maxg, per_loc = int(rng.integers(0, 14)), int(rng.integers(0, 11)), int(rng.integers(100, 2000))
+        got = tuple(int(v) for v in plan("octree %d %d %d %d %d %d %d %d\n" % (budget, fixed, window, depth, maxg, per_loc, leaf, tile))[0].split())
+        want = octree_plan_py(budget, fixed, window, depth, maxg, per_loc, leaf, tile)
+        assert got == want, (budget, fixed, window, depth, maxg, per_loc, leaf, tile)
+        if got[0] >= 0:  # the fixed set, the window, the selection, the block's images and a key batch stay within the budget
+            sel = (budget - fixed - window) // 8
+            assert got[0] <= min(depth, maxg) and sel // 2 >= got[2] * per_loc or got[2] == 1
+            assert fixed + window + sel + 40 * got[1] + block_bytes(got[0], depth - got[0], leaf, tile) + 5 * got[3] <= budget
 
 
 @pytest.mark.parametrize("seed", range(6))
