@@ -327,6 +327,32 @@ int pcv_xray_quadtree_from_dir_write_dir(pcv_ctx* ctx, const char* octree_dir, c
                                          const char* out_dir, pcv_xray_quadtree_info* info_out, pcv_xray_bounded_info* bounded_info_out,
                                          pcv_xray_dir_info* dir_info_out);
 
+/* ... with filter intervals on the intensity (closed, the attribute as f64): a leaf is made only of the points of its location
+ * that pass every interval, and a leaf whose location holds only points that fail does not exist.  The occupancy pass ignores
+ * the filters.  Filters on a directory without intensities -> PCV_ERR_INVALID; with a binned strategy -> PCV_ERR_UNSUPPORTED.
+ * nfilt = 0 is pcv_xray_quadtree_from_dir. */
+int pcv_xray_quadtree_from_dir_filtered(pcv_ctx* ctx, const char* octree_dir, const pcv_xray_quadtree_params* params, const pcv_interval* filters,
+                                        uint32_t nfilt, uint64_t max_device_bytes, pcv_xray_tile_fn on_tile, void* user, pcv_xray_quadtree_info* info_out,
+                                        pcv_xray_bounded_info* bounded_info_out, pcv_xray_dir_info* dir_info_out);
+int pcv_xray_quadtree_from_dir_filtered_write_dir(pcv_ctx* ctx, const char* octree_dir, const pcv_xray_quadtree_params* params, const pcv_interval* filters,
+                                                  uint32_t nfilt, uint64_t max_device_bytes, const char* out_dir, pcv_xray_quadtree_info* info_out,
+                                                  pcv_xray_bounded_info* bounded_info_out, pcv_xray_dir_info* dir_info_out);
+
+/* The X-ray quadtree of several resident octrees at once (build_xray_quadtree over a list of point_cloud_locations,
+ * point_cloud_client/src/lib.rs:118-141), with filter intervals on the intensity.  The quadtree lies over the union of the
+ * clouds' boxes (component-wise min and max, empty clouds included).  A leaf is made of every point of every cloud that its
+ * location contains and that passes every interval (closed, the attribute as f64); it exists iff one such point does.  XRay
+ * tiles do not depend on the clouds' order.  Delivery order, cancellation, the budget (the clouds' own arrays not counted) and
+ * the counters are those of pcv_xray_quadtree_bounded, which equals this call with n = 1 and no filters.  Errors: n = 0, a null
+ * cloud, clouds on different contexts, filters or the intensity strategy when a cloud has no intensities -> PCV_ERR_INVALID;
+ * a binned strategy with n > 1 or with filters -> PCV_ERR_UNSUPPORTED. */
+int pcv_xray_quadtree_clouds(const pcv_octree* const* octrees, uint32_t n, const pcv_xray_quadtree_params* params, const pcv_interval* filters, uint32_t nfilt,
+                             uint64_t max_device_bytes, pcv_xray_tile_fn on_tile, void* user, pcv_xray_quadtree_info* info_out,
+                             pcv_xray_bounded_info* bounded_info_out);
+int pcv_xray_quadtree_clouds_write_dir(const pcv_octree* const* octrees, uint32_t n, const pcv_xray_quadtree_params* params, const pcv_interval* filters,
+                                       uint32_t nfilt, uint64_t max_device_bytes, const char* directory, pcv_xray_quadtree_info* info_out,
+                                       pcv_xray_bounded_info* bounded_info_out);
+
 /* ---- point queries straight from an octree directory (Octree over OnDiskDataProvider, octree/mod.rs:156-215, 337-352) ---- */
 /* A directory-backed octree: open reads meta.pb into the node table pcv_octree_load_dir builds and puts its query tables on the
  * device; node files are only stat'ed.  Every call reads, uploads and culls only the nodes it selects, in chunks cut at 2048-point
@@ -448,6 +474,15 @@ int pcv_s2_xray_quadtree(const pcv_s2cloud* cloud, const pcv_xray_quadtree_param
 int pcv_s2_xray_quadtree_write_dir(const pcv_s2cloud* cloud, const pcv_xray_quadtree_params* params, const pcv_interval* filters, uint32_t nfilt,
                                    uint64_t max_device_bytes, const char* directory, pcv_xray_quadtree_info* info_out,
                                    pcv_xray_bounded_info* bounded_info_out);
+/* The X-ray quadtree of several resident S2 clouds at once, with the contract of pcv_xray_quadtree_clouds; also
+ * PCV_ERR_INVALID for XRAY_COLORED when a cloud has no colours, and PCV_ERR_UNSUPPORTED for every binned strategy.  n = 1 is
+ * pcv_s2_xray_quadtree. */
+int pcv_s2_xray_quadtree_clouds(const pcv_s2cloud* const* clouds, uint32_t n, const pcv_xray_quadtree_params* params, const pcv_interval* filters,
+                                uint32_t nfilt, uint64_t max_device_bytes, pcv_xray_tile_fn on_tile, void* user, pcv_xray_quadtree_info* info_out,
+                                pcv_xray_bounded_info* bounded_info_out);
+int pcv_s2_xray_quadtree_clouds_write_dir(const pcv_s2cloud* const* clouds, uint32_t n, const pcv_xray_quadtree_params* params, const pcv_interval* filters,
+                                          uint32_t nfilt, uint64_t max_device_bytes, const char* directory, pcv_xray_quadtree_info* info_out,
+                                          pcv_xray_bounded_info* bounded_info_out);
 /* CellUnion::contains for arbitrary points: mask_out[i] = union.contains_cellid(CellID::from_point(p_i)). */
 int pcv_s2_union_contains(pcv_ctx* ctx, const pcv_points* host_points, const uint64_t* union_ids, uint32_t n_union, uint8_t* mask_out);
 

@@ -18,6 +18,7 @@
 #include <functional>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "pcv.h"
@@ -111,6 +112,18 @@ struct PointQuery {  // iterator.rs:66-72 (attributes: colour is always delivere
     std::vector<ClosedInterval> filter_intervals;  // on "intensity"
 };
 
+namespace detail {
+// The tile callback of the X-ray quadtree entries over a C++ callable (level, index, RGBA, tile_px).
+template <class F>
+struct XrayThunk {
+    F* f;
+    static int call(void* user, uint8_t level, uint64_t index, const uint8_t* rgba, uint32_t tile_px) {
+        (*static_cast<XrayThunk*>(user)->f)(level, index, rgba, tile_px);
+        return 0;
+    }
+};
+}  // namespace detail
+
 class Context {
    public:
     explicit Context(int device = 0, uint64_t max_points_per_node = 0) {
@@ -127,15 +140,9 @@ class Context {
     pcv_xray_quadtree_info build_xray_quadtree_from_dir(const std::string& octree_dir, const pcv_xray_quadtree_params& params, F&& on_tile,
                                                         uint64_t max_device_bytes = 0, pcv_xray_bounded_info* bounded_info = nullptr,
                                                         pcv_xray_dir_info* dir_info = nullptr) const {
-        struct Thunk {
-            F* f;
-            static int call(void* user, uint8_t level, uint64_t index, const uint8_t* rgba, uint32_t tile_px) {
-                (*static_cast<Thunk*>(user)->f)(level, index, rgba, tile_px);
-                return 0;
-            }
-        } th{&on_tile};
+        detail::XrayThunk<std::remove_reference_t<F>> th{&on_tile};
         pcv_xray_quadtree_info info{};
-        check(pcv_xray_quadtree_from_dir(h_, octree_dir.c_str(), &params, max_device_bytes, &Thunk::call, &th, &info, bounded_info, dir_info));
+        check(pcv_xray_quadtree_from_dir(h_, octree_dir.c_str(), &params, max_device_bytes, &decltype(th)::call, &th, &info, bounded_info, dir_info));
         return info;
     }
 
@@ -258,15 +265,9 @@ class Octree {
     template <class F>
     pcv_xray_quadtree_info build_xray_quadtree(const pcv_xray_quadtree_params& params, F&& on_tile, uint64_t max_device_bytes = 0,
                                                pcv_xray_bounded_info* bounded_info = nullptr) const {
-        struct Thunk {
-            F* f;
-            static int call(void* user, uint8_t level, uint64_t index, const uint8_t* rgba, uint32_t tile_px) {
-                (*static_cast<Thunk*>(user)->f)(level, index, rgba, tile_px);
-                return 0;
-            }
-        } th{&on_tile};
+        detail::XrayThunk<std::remove_reference_t<F>> th{&on_tile};
         pcv_xray_quadtree_info info{};
-        check(pcv_xray_quadtree_bounded(o_, &params, max_device_bytes, &Thunk::call, &th, &info, bounded_info));
+        check(pcv_xray_quadtree_bounded(o_, &params, max_device_bytes, &decltype(th)::call, &th, &info, bounded_info));
         return info;
     }
     void write_to_directory(const std::string& dir) const { check(pcv_octree_write_dir(o_, dir.c_str())); }
@@ -595,16 +596,10 @@ class S2Cells {
     template <class F>
     pcv_xray_quadtree_info xray_quadtree(const pcv_xray_quadtree_params& params, const std::vector<ClosedInterval>& filter_intervals, F&& on_tile,
                                          uint64_t max_device_bytes = 0, pcv_xray_bounded_info* bounded_info = nullptr) const {
-        struct Thunk {
-            F* f;
-            static int call(void* user, uint8_t level, uint64_t index, const uint8_t* rgba, uint32_t tile_px) {
-                (*static_cast<Thunk*>(user)->f)(level, index, rgba, tile_px);
-                return 0;
-            }
-        } th{&on_tile};
+        detail::XrayThunk<std::remove_reference_t<F>> th{&on_tile};
         const std::vector<pcv_interval> f = detail::raw_intervals(filter_intervals);
         pcv_xray_quadtree_info info{};
-        check(pcv_s2_xray_quadtree(s_, &params, f.data(), (uint32_t)f.size(), max_device_bytes, &Thunk::call, &th, &info, bounded_info));
+        check(pcv_s2_xray_quadtree(s_, &params, f.data(), (uint32_t)f.size(), max_device_bytes, &decltype(th)::call, &th, &info, bounded_info));
         return info;
     }
     void write_to_directory(const std::string& dir) const { check(pcv_s2_write_dir(s_, dir.c_str())); }
@@ -613,6 +608,49 @@ class S2Cells {
    private:
     pcv_s2cloud* s_;
 };
+
+// build_xray_quadtree over several resident octrees at once (point_cloud_client/src/lib.rs:118-141): the quadtree over the union
+// of their boxes, every leaf made of the points of all of them that its location contains and that pass `filter_intervals`.
+// Tiles through `on_tile` in post-order, as Octree::build_xray_quadtree delivers them (pcv_xray_quadtree_clouds).
+template <class F>
+pcv_xray_quadtree_info build_xray_quadtree(const std::vector<const Octree*>& clouds, const pcv_xray_quadtree_params& params,
+                                           const std::vector<ClosedInterval>& filter_intervals, F&& on_tile, uint64_t max_device_bytes = 0,
+                                           pcv_xray_bounded_info* bounded_info = nullptr) {
+    std::vector<const pcv_octree*> raw;
+    for (const Octree* o : clouds) raw.push_back(o ? o->raw() : nullptr);
+    const std::vector<pcv_interval> f = detail::raw_intervals(filter_intervals);
+    detail::XrayThunk<std::remove_reference_t<F>> th{&on_tile};
+    pcv_xray_quadtree_info info{};
+    check(pcv_xray_quadtree_clouds(raw.data(), (uint32_t)raw.size(), &params, f.data(), (uint32_t)f.size(), max_device_bytes, &decltype(th)::call, &th, &info,
+                                   bounded_info));
+    return info;
+}
+// ... over several resident S2 clouds at once (pcv_s2_xray_quadtree_clouds).
+template <class F>
+pcv_xray_quadtree_info build_xray_quadtree(const std::vector<const S2Cells*>& clouds, const pcv_xray_quadtree_params& params,
+                                           const std::vector<ClosedInterval>& filter_intervals, F&& on_tile, uint64_t max_device_bytes = 0,
+                                           pcv_xray_bounded_info* bounded_info = nullptr) {
+    std::vector<const pcv_s2cloud*> raw;
+    for (const S2Cells* s : clouds) raw.push_back(s ? s->raw() : nullptr);
+    const std::vector<pcv_interval> f = detail::raw_intervals(filter_intervals);
+    detail::XrayThunk<std::remove_reference_t<F>> th{&on_tile};
+    pcv_xray_quadtree_info info{};
+    check(pcv_s2_xray_quadtree_clouds(raw.data(), (uint32_t)raw.size(), &params, f.data(), (uint32_t)f.size(), max_device_bytes, &decltype(th)::call, &th, &info,
+                                      bounded_info));
+    return info;
+}
+// Context::build_xray_quadtree_from_dir with filter intervals (pcv_xray_quadtree_from_dir_filtered).
+template <class F>
+pcv_xray_quadtree_info build_xray_quadtree_from_dir(const Context& ctx, const std::string& octree_dir, const pcv_xray_quadtree_params& params,
+                                                    const std::vector<ClosedInterval>& filter_intervals, F&& on_tile, uint64_t max_device_bytes = 0,
+                                                    pcv_xray_bounded_info* bounded_info = nullptr, pcv_xray_dir_info* dir_info = nullptr) {
+    const std::vector<pcv_interval> f = detail::raw_intervals(filter_intervals);
+    detail::XrayThunk<std::remove_reference_t<F>> th{&on_tile};
+    pcv_xray_quadtree_info info{};
+    check(pcv_xray_quadtree_from_dir_filtered(ctx.raw(), octree_dir.c_str(), &params, f.data(), (uint32_t)f.size(), max_device_bytes, &decltype(th)::call, &th,
+                                              &info, bounded_info, dir_info));
+    return info;
+}
 
 inline bool S2Cells::for_each_batch(const PointQuery& query, size_t batch_size, const std::function<bool(PointsBatch&&)>& func) const {
     const std::vector<pcv_interval> f = detail::raw_intervals(query.filter_intervals);

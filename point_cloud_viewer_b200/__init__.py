@@ -177,20 +177,45 @@ class Context:
 
     # -- X-ray quadtrees straight from an octree directory (never resident as a whole)
     def xray_quadtree_from_dir(self, octree_dir, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0,
-                               query_from_global=None, background=(255, 255, 255, 255), root=(0, 0), on_tile=None, keep_tiles=True, max_device_bytes=0):
+                               query_from_global=None, background=(255, 255, 255, 255), root=(0, 0), on_tile=None, keep_tiles=True, max_device_bytes=0,
+                               filter_intervals=()):
         """Octree.xray_quadtree over the octree in `octree_dir`, streamed from disk window by window: the same (info dict, tiles)
         and keywords.  `max_device_bytes` bounds everything the call allocates (0: most of the free memory); the info dict also
         holds the pcv_xray_dir_info fields."""
         pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
-        return _xray_call(N.lib().pcv_xray_quadtree_from_dir, (self.h, os.fsencode(str(octree_dir)), C.byref(pr), int(max_device_bytes)), True, True, on_tile,
-                          keep_tiles)
+        f, nf = _intervals(filter_intervals)
+        return _xray_call(N.lib().pcv_xray_quadtree_from_dir_filtered, (self.h, os.fsencode(str(octree_dir)), C.byref(pr), _p(f), nf, int(max_device_bytes)), True,
+                          True, on_tile, keep_tiles)
 
     def xray_quadtree_from_dir_write_dir(self, octree_dir, out_dir, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0,
-                                         query_from_global=None, background=(255, 255, 255, 255), root=(0, 0), max_device_bytes=0):
+                                         query_from_global=None, background=(255, 255, 255, 255), root=(0, 0), max_device_bytes=0, filter_intervals=()):
         """xray_quadtree_from_dir with the reference's outputs: <out_dir>/<node id>.png + the quadtree's meta file."""
         pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
-        return _xray_call(N.lib().pcv_xray_quadtree_from_dir_write_dir,
-                          (self.h, os.fsencode(str(octree_dir)), C.byref(pr), int(max_device_bytes), os.fsencode(str(out_dir))), True)
+        f, nf = _intervals(filter_intervals)
+        return _xray_call(N.lib().pcv_xray_quadtree_from_dir_filtered_write_dir,
+                          (self.h, os.fsencode(str(octree_dir)), C.byref(pr), _p(f), nf, int(max_device_bytes), os.fsencode(str(out_dir))), True)
+
+    # -- X-ray quadtrees over several resident clouds at once
+    def xray_quadtree_clouds(self, clouds, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0, query_from_global=None,
+                             background=(255, 255, 255, 255), root=(0, 0), on_tile=None, keep_tiles=True, filter_intervals=(), max_device_bytes=0):
+        """Octree.xray_quadtree over a list of Octree or a list of S2Cloud together (pcv_xray_quadtree_clouds,
+        pcv_s2_xray_quadtree_clouds): the quadtree over the union of their boxes, every leaf made of the points of all of them
+        that its location contains and that pass `filter_intervals` ((lo, hi) pairs on the intensity, closed).  Returns
+        (info dict, {(level, index): RGBA array}); the other keywords as in Octree.xray_quadtree."""
+        pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
+        f, nf = _intervals(filter_intervals)
+        octrees, hs = _cloud_handles(clouds)
+        fn = N.lib().pcv_xray_quadtree_clouds if octrees else N.lib().pcv_s2_xray_quadtree_clouds
+        return _xray_call(fn, (hs, len(clouds), C.byref(pr), _p(f), nf, int(max_device_bytes)), False, True, on_tile, keep_tiles)
+
+    def xray_quadtree_clouds_write_dir(self, clouds, out_dir, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0,
+                                       query_from_global=None, background=(255, 255, 255, 255), root=(0, 0), filter_intervals=(), max_device_bytes=0):
+        """xray_quadtree_clouds with the reference's outputs: <out_dir>/<node id>.png + the quadtree's meta file."""
+        pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
+        f, nf = _intervals(filter_intervals)
+        octrees, hs = _cloud_handles(clouds)
+        fn = N.lib().pcv_xray_quadtree_clouds_write_dir if octrees else N.lib().pcv_s2_xray_quadtree_clouds_write_dir
+        return _xray_call(fn, (hs, len(clouds), C.byref(pr), _p(f), nf, int(max_device_bytes), os.fsencode(str(out_dir))), False)
 
     def open_dir(self, directory, max_device_bytes=0):
         """An OctreeDir over the octree in `directory`: queries read only the nodes they select (0: most of the free memory)."""
@@ -619,19 +644,24 @@ class Octree:
         return bool(anyp.value), rgba
 
     def xray_quadtree(self, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0, query_from_global=None,
-                      background=(255, 255, 255, 255), root=(0, 0), on_tile=None, keep_tiles=True, max_device_bytes=0):
+                      background=(255, 255, 255, 255), root=(0, 0), on_tile=None, keep_tiles=True, max_device_bytes=0, filter_intervals=()):
         """build_xray_quadtree (xray/src/generation.rs:560-622) on the GPU: returns (info dict, {(level, index): RGBA array}).
         `on_tile(level, index, rgba)` is called for every finished tile in post-order, every tile after its children (return a
         true value to cancel).  `max_device_bytes` bounds the driver's device memory (0: most of the free memory); the info
-        dict holds the pcv_xray_quadtree_info and pcv_xray_bounded_info fields."""
+        dict holds the pcv_xray_quadtree_info and pcv_xray_bounded_info fields.  `filter_intervals`: (lo, hi) pairs on the
+        intensity (closed); a leaf is made only of the points that pass all of them."""
         pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
-        return _xray_call(N.lib().pcv_xray_quadtree_bounded, (self.h, C.byref(pr), int(max_device_bytes)), False, True, on_tile, keep_tiles)
+        f, nf = _intervals(filter_intervals)
+        return _xray_call(N.lib().pcv_xray_quadtree_clouds, ((C.c_void_p * 1)(self.h), 1, C.byref(pr), _p(f), nf, int(max_device_bytes)), False, True, on_tile,
+                          keep_tiles)
 
     def xray_quadtree_write_dir(self, directory, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0, query_from_global=None,
-                                background=(255, 255, 255, 255), root=(0, 0), max_device_bytes=0):
+                                background=(255, 255, 255, 255), root=(0, 0), max_device_bytes=0, filter_intervals=()):
         """build_xray_quadtree with the reference's outputs: <directory>/<node id>.png + the quadtree's meta file."""
         pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
-        return _xray_call(N.lib().pcv_xray_quadtree_bounded_write_dir, (self.h, C.byref(pr), int(max_device_bytes), os.fsencode(str(directory))), False)
+        f, nf = _intervals(filter_intervals)
+        return _xray_call(N.lib().pcv_xray_quadtree_clouds_write_dir,
+                          ((C.c_void_p * 1)(self.h), 1, C.byref(pr), _p(f), nf, int(max_device_bytes), os.fsencode(str(directory))), False)
 
 
 def _loc_arg(loc):
@@ -862,17 +892,15 @@ class S2Cloud:
         stored points its location contains that pass `filter_intervals` ((lo, hi) pairs on the intensity, closed).  Returns
         (info dict, {(level, index): RGBA array}); `on_tile` and `max_device_bytes` as in Octree.xray_quadtree."""
         pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
-        f = np.ascontiguousarray(np.asarray(filter_intervals, np.float64).reshape(-1))
-        return _xray_call(N.lib().pcv_s2_xray_quadtree, (self.h, C.byref(pr), _p(f) if len(f) else None, len(f) // 2, int(max_device_bytes)), False, True, on_tile,
-                          keep_tiles)
+        f, nf = _intervals(filter_intervals)
+        return _xray_call(N.lib().pcv_s2_xray_quadtree, (self.h, C.byref(pr), _p(f), nf, int(max_device_bytes)), False, True, on_tile, keep_tiles)
 
     def xray_quadtree_write_dir(self, directory, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0, query_from_global=None,
                                 background=(255, 255, 255, 255), root=(0, 0), filter_intervals=(), max_device_bytes=0):
         """xray_quadtree with the reference's outputs: <directory>/<node id>.png + the quadtree's meta file."""
         pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
-        f = np.ascontiguousarray(np.asarray(filter_intervals, np.float64).reshape(-1))
-        return _xray_call(N.lib().pcv_s2_xray_quadtree_write_dir,
-                          (self.h, C.byref(pr), _p(f) if len(f) else None, len(f) // 2, int(max_device_bytes), os.fsencode(str(directory))), False)
+        f, nf = _intervals(filter_intervals)
+        return _xray_call(N.lib().pcv_s2_xray_quadtree_write_dir, (self.h, C.byref(pr), _p(f), nf, int(max_device_bytes), os.fsencode(str(directory))), False)
 
 
 def s2_token(cell_id):
@@ -903,6 +931,26 @@ def _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_siz
     pr.tile_size_px, pr.pixel_size_m = int(tile_size_px), float(pixel_size_m)
     pr.root_level, pr.root_index = int(root[0]), int(root[1])
     return pr
+
+
+def _intervals(filter_intervals):
+    """(lo, hi) pairs -> (contiguous float64 array of pcv_interval or None, count)."""
+    f = np.ascontiguousarray(np.asarray(filter_intervals, np.float64).reshape(-1))
+    return (f if len(f) else None), len(f) // 2
+
+
+def _cloud_handles(clouds):
+    """A list of Octree or a list of S2Cloud -> (is octrees, C array of their handles); a mixed or empty list raises."""
+    clouds = list(clouds)
+    if not clouds:
+        raise ValueError("xray_quadtree_clouds needs at least one cloud")
+    if all(isinstance(c, Octree) for c in clouds):
+        octrees = True
+    elif all(isinstance(c, S2Cloud) for c in clouds):
+        octrees = False
+    else:
+        raise TypeError("clouds must all be Octree or all be S2Cloud")
+    return octrees, (C.c_void_p * len(clouds))(*[c.h for c in clouds])
 
 
 def _xray_call(fn, args, dir_info, with_tiles=False, on_tile=None, keep_tiles=True):

@@ -232,6 +232,14 @@ SYMBOLS = [
                                              C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo), C.POINTER(XrayDirInfo)]),
     ("pcv_xray_quadtree_from_dir_write_dir", C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(XrayQuadtreeParams), C.c_uint64, C.c_char_p,
                                                        C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo), C.POINTER(XrayDirInfo)]),
+    ("pcv_xray_quadtree_from_dir_filtered", C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64, XRAY_TILE_FN,
+                                                      C.c_void_p, C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo), C.POINTER(XrayDirInfo)]),
+    ("pcv_xray_quadtree_from_dir_filtered_write_dir", C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64,
+                                                                C.c_char_p, C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo), C.POINTER(XrayDirInfo)]),
+    ("pcv_xray_quadtree_clouds", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64, XRAY_TILE_FN, C.c_void_p,
+                                           C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo)]),
+    ("pcv_xray_quadtree_clouds_write_dir", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64, C.c_char_p,
+                                                     C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo)]),
     ("pcv_octree_dir_open", C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, C.POINTER(C.c_void_p)]),
     ("pcv_octree_dir_close", None, [C.c_void_p]),
     ("pcv_octree_dir_info", C.c_int, [C.c_void_p, _u64p, _u64p, _u64p, _dp, _dp, _dp, C.POINTER(C.c_int)]),
@@ -266,6 +274,10 @@ SYMBOLS = [
                                        C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo)]),
     ("pcv_s2_xray_quadtree_write_dir", C.c_int, [C.c_void_p, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64, C.c_char_p,
                                                  C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo)]),
+    ("pcv_s2_xray_quadtree_clouds", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64, XRAY_TILE_FN,
+                                              C.c_void_p, C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo)]),
+    ("pcv_s2_xray_quadtree_clouds_write_dir", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64,
+                                                        C.c_char_p, C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo)]),
     ("pcv_s2_union_contains", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_void_p, C.c_uint32, C.c_void_p]),
     ("pcv_prefix_histogram_device", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_double, _dp, _dp, C.c_uint32, C.c_void_p]),
     ("pcv_prefix_histogram_bbox_device", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_double, _dp, _dp, C.c_uint32, C.c_void_p, _dp, _dp]),

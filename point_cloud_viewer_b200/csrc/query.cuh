@@ -816,11 +816,25 @@ struct XrayBinArgs {
     uint32_t* sub_cursor;     // [nsub] place pass: keys written so far
     uint32_t* keys;           // ly << 16 | lx << 11 | min(z, 1024)
 };
+// The filter intervals of the octree X-ray kernels: point `slot` takes part iff lo <= (double)intensity[slot] <= hi for every
+// interval (closed, the attribute as f64: iterator.rs:82-91, as point_passes and s2_leaf_hits test it).
+struct XrayFilt {
+    const float* intensity;  // node-contiguous intensities
+    const pcv_interval* filters;
+    uint32_t nfilt;
+};
+__device__ __forceinline__ bool xray_filt_pass(const XrayFilt& f, uint64_t slot) {
+    const double v = (double)f.intensity[slot];
+    for (uint32_t k = 0; k < f.nfilt; ++k)
+        if (!(f.filters[k].lo <= v && v <= f.filters[k].hi)) return false;
+    return true;
+}
 // The count (PLACE = 0) or place (PLACE = 1) pass over work tile t of the image of `a`: every point drawn into the image goes
-// to bin bin0 + its sub-tile.  Returns whether one of the thread's points passed the location test.
-template <int PLACE>
+// to bin bin0 + its sub-tile.  Returns whether one of the thread's points passed the location test.  FILT: only points that
+// pass `f` take part (a point that fails gets no key and does not count as seen).
+template <int PLACE, bool FILT = false>
 __device__ __forceinline__ bool xray_bin_tile(const XrayArgs& a, const QNode* nodes, const uint8_t* xyz, const QTile t, uint32_t bin0, uint32_t sub_w,
-                                              uint32_t* sub_count, uint32_t* sub_cursor, uint32_t* keys) {
+                                              uint32_t* sub_count, uint32_t* sub_cursor, uint32_t* keys, const XrayFilt& f) {
     const int lane = threadIdx.x & 31;
     const QNode nd = nodes[t.node];
     const int bpc = enc_bytes(nd.enc);
@@ -831,7 +845,7 @@ __device__ __forceinline__ bool xray_bin_tile(const XrayArgs& a, const QNode* no
         if (i < t.count) {
             double p[3];
             decode_point(xyz, nd, bpc, t.first + i, p);
-            if (loc_contains(a.geom, p[0], p[1], p[2])) {
+            if ((!FILT || xray_filt_pass(f, nd.point_off + t.first + i)) && loc_contains(a.geom, p[0], p[1], p[2])) {
                 seen = true;
                 uint32_t x, y, z;
                 xray_pixel(a, p, x, y, z);
@@ -861,13 +875,15 @@ __device__ __forceinline__ bool xray_bin_tile(const XrayArgs& a, const QNode* no
 template <int PLACE>
 __global__ void __launch_bounds__(256) k_xray_bin(const __grid_constant__ XrayBinArgs b) {
     for (uint32_t ti = blockIdx.x; ti < b.ntiles; ti += gridDim.x)
-        xray_bin_tile<PLACE>(b.x, b.x.nodes, b.x.xyz, b.x.tiles[ti], 0, b.sub_w, b.sub_count, b.sub_cursor, b.keys);
+        xray_bin_tile<PLACE>(b.x, b.x.nodes, b.x.xyz, b.x.tiles[ti], 0, b.sub_w, b.sub_count, b.sub_cursor, b.keys, XrayFilt{});
 }
 // The same binning for a batch of leaf tiles of one quadtree (the bounded quadtree driver, xray_api.inl): every work tile
 // carries its leaf in `loc`, every leaf has its own location and box (leaves[loc]; transform, w and h are shared), and the bins
 // are (leaf, sub-tile) pairs, leaf-major: bin = leaf * nsub + sub.  A point on an edge shared by two leaves goes into every
 // leaf whose closed box contains it (the work list holds one tile per (leaf, node) pair).  The count pass also raises
 // seen[leaf] for every point that passes the leaf's location test: the leaf exists iff one does (generation.rs:489-504).
+// Several octrees bin into the same bins: each runs its count pass into sub_count, then after one scan its place pass through
+// the shared sub_cursor (the keys of a bin may come in any order).  FILT: only points that pass `filt` take part.
 struct XrayBatchArgs {
     const XrayArgs* leaves;   // [nleaf] geom, tmin, tdiag, rdiag, div_ok, query_from_global, has_q, w, h of every leaf
     const QNode* nodes;
@@ -879,12 +895,13 @@ struct XrayBatchArgs {
     uint32_t* sub_cursor;     // [nleaf * nsub]
     uint32_t* keys;
     int* seen;                // [nleaf]
+    XrayFilt filt;            // FILT only
 };
-template <int PLACE>
+template <int PLACE, bool FILT>
 __global__ void __launch_bounds__(256) k_xray_bin_batch(const __grid_constant__ XrayBatchArgs b) {
     for (uint32_t ti = blockIdx.x; ti < b.ntiles; ti += gridDim.x) {
         const QTile t = b.tiles[ti];
-        const bool seen = xray_bin_tile<PLACE>(b.leaves[t.loc], b.nodes, b.xyz, t, t.loc * b.nsub, b.sub_w, b.sub_count, b.sub_cursor, b.keys);
+        const bool seen = xray_bin_tile<PLACE, FILT>(b.leaves[t.loc], b.nodes, b.xyz, t, t.loc * b.nsub, b.sub_w, b.sub_count, b.sub_cursor, b.keys, b.filt);
         if (!PLACE && __syncthreads_or(seen) && threadIdx.x == 0) b.seen[t.loc] = 1;
     }
 }
@@ -1091,6 +1108,7 @@ struct XrayAttrArgs {
     double* dsum;            // mode 3: npix * 2
     unsigned long long* pivot;  // mode 3: npix, the bits of the column's pivot z; kPivotEmpty until a point claims it
     uint32_t* count;
+    XrayFilt filt;           // FILT only
 };
 constexpr unsigned long long kPivotEmpty = 0x7FF8DEADBEEF0000ull;  // a NaN payload no decoded coordinate carries
 // The column's pivot: the z of the first point to claim it with one CAS; every later point reads it.
@@ -1103,7 +1121,8 @@ __device__ __forceinline__ double xray_pivot(unsigned long long* slot, double z)
     return __longlong_as_double((long long)cur);
 }
 
-template <int MODE>
+// FILT: only points that pass b.filt take part (a point that fails adds nothing and does not count as seen).
+template <int MODE, bool FILT>
 __global__ void __launch_bounds__(256) k_xray_accum_attr(const __grid_constant__ XrayAttrArgs b) {
     const XrayArgs& a = b.x;
     const QTile t = a.tiles[blockIdx.x];
@@ -1113,6 +1132,7 @@ __global__ void __launch_bounds__(256) k_xray_accum_attr(const __grid_constant__
     for (uint32_t i = threadIdx.x; i < t.count; i += blockDim.x) {
         double p[3];
         decode_point(a.xyz, nd, bpc, t.first + i, p);
+        if (FILT && !xray_filt_pass(b.filt, nd.point_off + t.first + i)) continue;
         if (!loc_contains(a.geom, p[0], p[1], p[2])) continue;
         seen = true;
         uint32_t x, y, z;

@@ -4,6 +4,7 @@
 //   xray_levels_to_close: the post-order bookkeeping - which ancestors are complete when the walk moves on to the next subtree
 //   xray_post_order:      every node of a subtree with the given leaves, each after all of its children
 //   xray_octree_plan:     the octree sources' plan: block depth, node selection and key capacity
+//   xray_clouds_fixed_bytes: what a list of resident octrees holds for the whole run besides the driver's own fixed set
 //   s2_xray_plan:         the S2 cloud's leaf producer (s2_xray.inl): block depth, key capacity and attribute batch size
 #pragma once
 #include <algorithm>
@@ -90,21 +91,34 @@ struct XrayPlan {
 
 // The plan of an octree source: `fixed` bytes for the whole run and `window` bytes of points (0 for a resident octree; the
 // largest window of the blocks for an octree directory).  An eighth of what they leave goes to the node selection (half to
-// its frontier, `sel_cap` pairs and 40 B more per pair, half to `max_loc` locations of `per_loc` bytes); g is the largest
-// block depth <= max_g whose images fit besides; what remains after the block's images holds the keys of a batch, 4 bytes per
-// key and its share of the work tiles.
+// its frontier, `sel_cap` pairs and `xray_pair_bytes(clouds)` more per pair, half to `max_loc` locations of `per_loc` bytes); g
+// is the largest block depth <= max_g whose images fit besides; what remains after the block's images holds the keys of a
+// batch, 4 bytes per key and its share of the work tiles.
+// A pair costs 24 B of frontier and 16 B of work list.  `clouds` octrees select in turn, each frontier released before the
+// next selection, but every cloud's work list stays until the batch's place passes: 24 + 16 clouds bytes per pair.
+inline uint64_t xray_pair_bytes(uint32_t clouds) { return 24 + 16ull * clouds; }
 inline XrayPlan xray_octree_plan(uint64_t budget, uint64_t fixed, uint64_t window, int depth, int max_g, uint64_t per_loc, uint64_t leaf_bytes,
-                                 uint64_t tile_bytes) {
+                                 uint64_t tile_bytes, uint32_t clouds = 1) {
     XrayPlan p;
+    const uint64_t pair = xray_pair_bytes(clouds);
     const uint64_t sel_bytes = budget > fixed + window ? (budget - fixed - window) / 8 : 0;
-    p.sel_cap = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(sel_bytes / 2 / 40, 64), 48ull << 20);
+    p.sel_cap = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(sel_bytes / 2 / pair, 64), 48ull << 20);
     p.max_loc = std::max<uint64_t>(1, sel_bytes / 2 / per_loc);
-    const uint64_t held = fixed + window + sel_bytes + 40ull * p.sel_cap;
+    const uint64_t held = fixed + window + sel_bytes + pair * p.sel_cap;
     p.g = xray_block_depth(budget, held, depth, max_g, leaf_bytes, tile_bytes);
     if (p.g < 0) return p;
     const uint64_t used = held + xray_block_bytes(p.g, depth - p.g, leaf_bytes, tile_bytes);
     p.key_cap = budget > used ? std::min<uint64_t>((budget - used) / 5, 0xFFFFFFFEull) : 0;
     return p;
+}
+
+// The fixed bytes of resident octrees (xray_octree_plan's `fixed`): the driver's own fixed set `run_fixed`, each cloud's work
+// list of every node for the pruning pass (16 B per tile and 16 B more), and the filter intervals (16 B each).  The clouds'
+// frontiers and work lists of a key batch are counted per selection pair by xray_octree_plan (xray_pair_bytes).
+inline uint64_t xray_clouds_fixed_bytes(uint64_t run_fixed, const std::vector<uint64_t>& cloud_tiles, uint32_t nfilt) {
+    uint64_t fixed = run_fixed + 16ull * nfilt;
+    for (uint64_t t : cloud_tiles) fixed += 16 * t + 16;
+    return fixed;
 }
 
 // ---- the leaf producer of an S2 cloud (s2_xray.inl) --------------------------------------------------------------------------
