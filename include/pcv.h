@@ -73,8 +73,12 @@ typedef struct pcv_node_meta {
     uint64_t xyz_byte_offset; /* first byte of the node's .xyz content                           */
 } pcv_node_meta;
 
-/* PointLocation (src/iterator.rs:13-20).  Same field layout as the oracle's orc_location. */
-enum { PCV_LOC_ALL = 0, PCV_LOC_AABB = 1, PCV_LOC_FRUSTUM = 2, PCV_LOC_OBB = 3 };
+/* PointLocation (src/iterator.rs:13-20).  Same field layout as the oracle's orc_location.
+ * PCV_LOC_WEB_MERCATOR_RECT (web_mercator_rect.rs) keeps north_west in aabb_min[0..1] and south_east in aabb_max[0..1], both
+ * normalised to [0, 1) as pcv_web_mercator_rect leaves them; every other field is zero.  A kind-4 location the constructor
+ * could not have made (non-finite or outside [0, 1), north_west.y > south_east.y, or more than one zoom-0 pixel across) is
+ * PCV_ERR_INVALID for every query. */
+enum { PCV_LOC_ALL = 0, PCV_LOC_AABB = 1, PCV_LOC_FRUSTUM = 2, PCV_LOC_OBB = 3, PCV_LOC_WEB_MERCATOR_RECT = 4 };
 typedef struct pcv_location {
     int32_t kind;
     int32_t pad;
@@ -146,6 +150,17 @@ int pcv_octree_load_dir(pcv_ctx* ctx, const char* dir, pcv_octree** out); /* Oct
 /* ---- a11-a14: nodes_in_location (octree/mod.rs:309-323, octree_iterator.rs:30-43) ---------- */
 int pcv_nodes_in_location(const pcv_octree* o, const pcv_location* loc, uint64_t* ids_hi_lo, uint64_t cap, uint64_t* n_out);
 
+/* ---- PointLocation::WebMercatorRect (src/geometry/web_mercator_rect.rs), host only ------------------------------------------
+ * pcv_web_mercator_rect: WebMercatorRect::from_zoomed_coordinates(min, max, z) as a kind-4 location.  PCV_ERR_INVALID where the
+ * reference returns None (z > 23, a corner component < 0 or >= 256 * 2^z, (max - min) / 2^z with x rem_euclid 256 > 1, y > 1
+ * or y < 0) and for non-finite input.  x may wrap around the antimeridian (min.x > max.x); such a rect selects nodes but
+ * contains no point.
+ * pcv_web_mercator_coord: the map position of an ECEF point at zoom z, in [0, 256 * 2^z)^2 (x east, y south):
+ * WebMercatorCoord::from_lat_lng(ECEF -> WGS84).to_zoomed_coordinate(z), with the arithmetic of the cull kernels' point test.
+ * PCV_ERR_INVALID for z > 23. */
+int pcv_web_mercator_rect(const double min[2], const double max[2], uint32_t z, pcv_location* out);
+int pcv_web_mercator_coord(const double ecef[3], uint32_t z, double out[2]);
+
 /* ---- a17: Octree::get_visible_nodes (octree/mod.rs:228-283) --------------------------------- */
 int pcv_visible_nodes(const pcv_octree* o, const double clip_from_world[16], uint64_t* ids_hi_lo, uint64_t cap, uint64_t* n_out);
 
@@ -153,8 +168,9 @@ int pcv_visible_nodes(const pcv_octree* o, const double clip_from_world[16], uin
 /* Streams every point of every node in `loc` that passes the culling + interval filters, re-chunked
  * into batches of exactly batch_size points (last one short), on the caller's thread.
  * The argument contract holds for all three sources (octree, octree directory, S2 cloud) and their nodes / cells, stream and
- * batch calls: a location kind outside PCV_LOC_ALL..PCV_LOC_OBB, nfilt > 0 with filters == NULL, or filters over points
- * without intensity is PCV_ERR_INVALID; a callback that returns non-zero ends the stream with PCV_ERR_CANCELLED. */
+ * batch calls: a location kind outside PCV_LOC_ALL..PCV_LOC_WEB_MERCATOR_RECT, an invalid kind-4 rect, nfilt > 0 with
+ * filters == NULL, or filters over points without intensity is PCV_ERR_INVALID; a callback that returns non-zero ends the
+ * stream with PCV_ERR_CANCELLED. */
 int pcv_query_points(const pcv_octree* o, const pcv_location* loc, const pcv_interval* filters, uint32_t nfilt,
                      uint64_t batch_size, pcv_batch_cb cb, void* user);
 /* Throughput form: nloc locations in one call; survivors stay compacted in HBM.  counts_out[i] =
@@ -427,8 +443,8 @@ int pcv_s2_cells_in_union(const pcv_s2cloud* cloud, const uint64_t* union_ids, u
  * input order inside a cell.  n_out = number of survivors (may exceed cap: only cap are written). */
 int pcv_s2_query_union(const pcv_s2cloud* cloud, const uint64_t* union_ids, uint32_t n_union, double* xyz_out, uint8_t* rgb_out,
                        float* intensity_out, uint64_t* src_index_out, uint64_t cap, uint64_t* n_out, uint64_t* tested_out);
-/* Every PointLocation except WebMercatorRect, with interval filters, streamed or batched on the GPU.  A cell's point box is the
- * exact component-wise min and max of its stored positions.  AllPoints selects every cell; Aabb, Obb and Frustum select the
+/* Every PointLocation, with interval filters, streamed or batched on the GPU.  A cell's point box is the exact component-wise
+ * min and max of its stored positions.  AllPoints selects every cell; Aabb, Obb, Frustum and WebMercatorRect select the
  * cells whose point box the location's separating-axis test (cache_separating_axes_for_aabb, sat.rs) does not call Out (a cell
  * without points has no box and is never selected); a cell union selects the cells whose id range intersects it.  This cell
  * list is not the reference's (which selects through latitude / longitude rectangles); the points are a superset of the

@@ -102,7 +102,21 @@ struct PointLocation {
         for (int i = 0; i < 3; ++i) l.raw.half_extent[i] = half_extent[i];
         return l;
     }
+    // WebMercatorRect::from_zoomed_coordinates(min, max, z) (web_mercator_rect.rs:40-53), map pixels at zoom z; throws
+    // Error(PCV_ERR_INVALID) where the reference returns None.
+    static PointLocation WebMercatorRect(const std::array<double, 2>& min, const std::array<double, 2>& max, uint32_t z) {
+        PointLocation l;
+        check(pcv_web_mercator_rect(min.data(), max.data(), z, &l.raw));
+        return l;
+    }
 };
+
+// WebMercatorCoord::from_lat_lng(ECEF -> WGS84).to_zoomed_coordinate(z): an ECEF point's map pixel at zoom z.
+inline std::array<double, 2> web_mercator_coord(const std::array<double, 3>& ecef, uint32_t z) {
+    std::array<double, 2> out{};
+    check(pcv_web_mercator_coord(ecef.data(), z, out.data()));
+    return out;
+}
 
 struct ClosedInterval {
     double lower_bound, upper_bound;

@@ -209,6 +209,8 @@ SYMBOLS = [
     ("pcv_octree_write_dir", C.c_int, [C.c_void_p, C.c_char_p]),
     ("pcv_octree_load_dir", C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),
     ("pcv_nodes_in_location", C.c_int, [C.c_void_p, C.POINTER(Location), C.c_void_p, C.c_uint64, _u64p]),
+    ("pcv_web_mercator_rect", C.c_int, [_dp, _dp, C.c_uint32, C.POINTER(Location)]),
+    ("pcv_web_mercator_coord", C.c_int, [_dp, C.c_uint32, _dp]),
     ("pcv_visible_nodes", C.c_int, [C.c_void_p, _dp, C.c_void_p, C.c_uint64, _u64p]),
     ("pcv_query_points", C.c_int, [C.c_void_p, C.POINTER(Location), C.c_void_p, C.c_uint32, C.c_uint64, BATCH_CB, C.c_void_p]),
     ("pcv_query_batch_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),

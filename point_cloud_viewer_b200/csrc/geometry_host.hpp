@@ -4,12 +4,14 @@
 //   Frustum corners/edges/normals   src/geometry/frustum.rs:129-166
 //   Obb corners/edges               src/geometry/obb.rs:49-78
 //   Aabb fast path (3 unit axes)    src/geometry/aabb.rs:103-111
+//   WebMercatorRect                 src/geometry/web_mercator_rect.rs:40-127, src/math/web_mercator.rs:38-97
 //   axis generation + O(n^2) dedup  src/math/sat.rs:80-143
 //   Matrix4::transform_point        nalgebra 0.22 (column-by-column accumulation, divide by w if != 0)
 #pragma once
 #include <cmath>
 #include <cstring>
 #include <limits>
+#include <stdexcept>
 
 #include "../../include/pcv.h"
 #include "s2.h"
@@ -61,24 +63,107 @@ PCV_GHD V3 iso_apply(const double* iso7, V3 p) {
     return V3{r.x + iso7[0], r.y + iso7[1], r.z + iso7[2]};
 }
 
+// ---- Web Mercator (src/math/web_mercator.rs) over the WGS84 ellipsoid ----------------------------------------------------
+// WGS84's defining semi-major axis and flattening; the semi-minor axis and the first eccentricity squared follow from them.
+constexpr double kWgs84A = 6378137.0;
+constexpr double kWgs84F = 1.0 / 298.257223563;
+constexpr double kWgs84B = kWgs84A * (1.0 - kWgs84F);
+constexpr double kWgs84E2 = 1.0 - (kWgs84B * kWgs84B) / (kWgs84A * kWgs84A);
+constexpr double kPi = 3.14159265358979323846;                // std::f64::consts::PI
+constexpr double kFrac1Pi = 0.31830988618379067153776752674503; // std::f64::consts::FRAC_1_PI
+constexpr double kWmLatBoundRad = 1.4844222297453324;          // LAT_BOUND_RAD: 2 atan(e^pi) - pi/2, 85.051129 degrees
+constexpr double kWmLatBoundSin = 0.99627207622075;            // LAT_BOUND_SIN = sin(LAT_BOUND_RAD)
+constexpr uint32_t kWmMaxZoom = 23;                            // MAX_ZOOM: 256 << z fits a u32
+constexpr double kWmMinElevation = -500.0;                     // the rect's extrusion, web_mercator_rect.rs:11-26
+constexpr double kWmMaxElevation = 10000.0;
+
+// nalgebra::clamp: min for NaN.
+PCV_GHD double wm_clamp(double v, double lo, double hi) { return v > lo ? (v < hi ? v : hi) : lo; }
+
+// ECEF -> WGS84 latitude and longitude (radians), the closed form of Heikkinen (1982) that the conversion literature calls
+// "Ferrari's solution"; the height is not needed.  Shared by the cull kernels and the host.
+PCV_GHD void ecef_to_lat_lng(double x, double y, double z, double& lat, double& lng) {
+    const double a2 = kWgs84A * kWgs84A, b2 = kWgs84B * kWgs84B, e2 = kWgs84E2, ep2 = (a2 - b2) / b2;
+    const double r2 = x * x + y * y, r = sqrt(r2), z2 = z * z;
+    const double f = 54.0 * b2 * z2;
+    const double g = r2 + (1.0 - e2) * z2 - e2 * (a2 - b2);
+    const double c = e2 * e2 * f * r2 / (g * g * g);
+    const double s = cbrt(1.0 + c + sqrt(c * c + 2.0 * c));
+    const double k = s + 1.0 / s + 1.0;
+    const double p = f / (3.0 * k * k * g * g);
+    const double q = sqrt(1.0 + 2.0 * e2 * e2 * p);
+    // the radicand is 0 on the polar axis in exact arithmetic and may round below it there
+    const double r0 = -(p * e2 * r) / (1.0 + q) + sqrt(fmax(0.5 * a2 * (1.0 + 1.0 / q) - p * (1.0 - e2) * z2 / (q * (1.0 + q)) - 0.5 * p * r2, 0.0));
+    const double t = r - e2 * r0;
+    const double v = sqrt(t * t + (1.0 - e2) * z2);
+    const double z0 = b2 * z / (kWgs84A * v);
+    lat = atan((z + ep2 * z0) / r);
+    lng = atan2(y, x);
+}
+
+// WebMercatorCoord::from_lat_lng (web_mercator.rs:38-50): the normalised map position in [0, 1)^2 (x east, y south).
+PCV_GHD void web_mercator_from_lat_lng(double lat, double lng, double w[2]) {
+    const double sin_y = sin(wm_clamp(lat, -kWmLatBoundRad, kWmLatBoundRad));
+    w[0] = 0.5 + lng / (2.0 * kPi);
+    w[1] = 0.5 - log((1.0 + sin_y) / (1.0 - sin_y)) * (0.25 * kFrac1Pi);
+}
+
+// WebMercatorRect::contains (web_mercator_rect.rs:121-127): the point's map position lies in [nw, se) component by component,
+// so a rect that wraps the antimeridian (nw.x > se.x) holds no point.  The point's altitude plays no part.
+PCV_GHD bool web_mercator_rect_contains(const double nw[2], const double se[2], double x, double y, double z) {
+    double lat, lng, w[2];
+    ecef_to_lat_lng(x, y, z, lat, lng);
+    web_mercator_from_lat_lng(lat, lng, w);
+    return nw[0] <= w[0] && nw[1] <= w[1] && w[0] < se[0] && w[1] < se[1];
+}
+
 // The kind of a QueryGeom built from a cell union (PointLocation::S2Cells, src/iterator.rs:13-20).  Internal: pcv_location has no
 // such kind; the cell-union entry points build the geometry themselves.
 constexpr int32_t kLocCellUnion = 16;
 
+// The most separating axes a location caches against an Aabb (sat.rs:111-142): 6 face normals, the 3 unit axes and the 12 x 3
+// edge cross products of a polyhedron with 12 edges (the Web Mercator rect's extrusion).
+constexpr int kMaxAxes = 6 + 3 + 12 * 3;
+// The axes a QueryGeom holds itself: every Aabb, Obb and Frustum (at most 5 + 3 + 6 x 3).  A Web Mercator rect's axes past these
+// live in a table its record points to (like a cell union's ids), so the record - one per location in every selection, X-ray
+// leaves included - keeps its size, and so do the projection tables (LocProj) and the kernels' shared-memory copies of them.
+constexpr int kInlineAxes = 26;
+struct MoreAxes {
+    double a[kMaxAxes - kInlineAxes][3];
+    double proj[kMaxAxes - kInlineAxes][2];  // the location's own projections on them (project_location_axis)
+};
+
 // What the device needs per location.
 struct QueryGeom {
     int32_t kind;
-    int32_t naxes;       // cached separating axes (<= 26); 0 for AllPoints and cell unions
-    double axes[26][3];
+    int32_t naxes;       // cached separating axes (<= kMaxAxes; past kInlineAxes in more_axes); 0 for AllPoints and cell unions
+    double axes[kInlineAxes][3];
     double corners[8][3];
-    double aabb_min[3], aabb_max[3];
+    double aabb_min[3], aabb_max[3];  // Web Mercator rect: north_west in aabb_min[0..1], south_east in aabb_max[0..1], as given
     double clip_from_query[16];
     double obb_from_query[7];
     double half_extent[3];
-    const uint64_t* cells;     // cell union: its normalised ids (device) ...
+    union {
+        const uint64_t* cells;      // cell union: its normalised ids (device) ...
+        const MoreAxes* more_axes;  // Web Mercator rect: its axes kInlineAxes.. (device for the kernels, host on the host)
+    };
     const S2Square* squares;   // ... and each one's face and square of leaf cells (device)
     uint32_t ncells, pad;
 };
+
+// Cached axis k of a location.
+PCV_GHD const double* geom_axis(const QueryGeom& g, int k) { return k < kInlineAxes ? g.axes[k] : g.more_axes->a[k - kInlineAxes]; }
+// The location's own projection on its axis k (project_location of query.cuh, one axis).
+PCV_GHD void project_location_axis(const QueryGeom& g, int k, double& lo, double& hi) {
+    const double* ax = geom_axis(g, k);
+    lo = 1.7976931348623157e308;
+    hi = -1.7976931348623157e308;
+    for (int i = 0; i < 8; ++i) {
+        const double p = g.corners[i][0] * ax[0] + g.corners[i][1] * ax[1] + g.corners[i][2] * ax[2];
+        lo = fmin(lo, p);
+        hi = fmax(hi, p);
+    }
+}
 
 inline V3 unit(V3 v) {
     const double n = std::sqrt(v3dot(v, v));
@@ -131,8 +216,76 @@ inline PolyIntersector obb_intersector(const double* query_from_obb, const doubl
     return r;
 }
 
+// WebMercatorCoord::to_lat_lng (web_mercator.rs:55-64).
+inline void web_mercator_to_lat_lng(const double w[2], double& lat, double& lng) {
+    const double cx = w[0] - 0.5, cy = w[1] - 0.5;
+    const double sin_term = std::exp(-cy * (4.0 * kPi));
+    const double one_over_sin_y = (sin_term + 1.0) * -0.5;
+    const double sin_y = wm_clamp(1.0 / one_over_sin_y + 1.0, -kWmLatBoundSin, kWmLatBoundSin);
+    lng = wm_clamp(cx * (2.0 * kPi), -kPi, kPi);
+    lat = std::asin(sin_y);
+}
+
+// WGS84 (latitude, longitude, height) -> ECEF.
+inline V3 wgs84_to_ecef(double lat, double lng, double h) {
+    const double sl = std::sin(lat), cl = std::cos(lat);
+    const double n = kWgs84A / std::sqrt(1.0 - kWgs84E2 * sl * sl);
+    return V3{(n + h) * cl * std::cos(lng), (n + h) * cl * std::sin(lng), (n * (1.0 - kWgs84E2) + h) * sl};
+}
+
+// A Web Mercator rect as the constructor leaves it (web_mercator_rect.rs:40-53, web_mercator.rs:84-97): both corners in
+// [0, 1), se.y >= nw.y, and at most one zoom-0 pixel across, where x may wrap around the antimeridian.  NaN fails.
+inline bool web_mercator_rect_valid(const double nw[2], const double se[2]) {
+    for (int i = 0; i < 2; ++i)
+        if (!(nw[i] >= 0.0 && nw[i] < 1.0 && se[i] >= 0.0 && se[i] < 1.0)) return false;
+    // (max - min) / 2^z of the constructor, exactly: its corners are these times 256 * 2^z
+    const double dx = (se[0] - nw[0]) * 256.0, dy = (se[1] - nw[1]) * 256.0;
+    double rx = std::fmod(dx, 256.0);  // f64::rem_euclid
+    if (rx < 0.0) rx += 256.0;
+    return !(rx > 1.0 || dy > 1.0 || dy < 0.0);
+}
+
+// WebMercatorRect::from_zoomed_coordinates: false where the reference returns None, and for non-finite input.
+inline bool web_mercator_rect_from_zoomed(const double mn[2], const double mx[2], uint32_t z, double nw[2], double se[2]) {
+    if (z > kWmMaxZoom) return false;
+    const double zoom = (double)(256u << z);
+    for (int i = 0; i < 2; ++i) {
+        nw[i] = mn[i] / zoom;  // powers of two: exact
+        se[i] = mx[i] / zoom;
+    }
+    return web_mercator_rect_valid(nw, se);
+}
+
+// WebMercatorRect::intersector (web_mercator_rect.rs:60-119): the rect's corners extruded from -500 m to 10 km, NW NE SE SW down,
+// then up; 12 edges and 6 face normals.
+inline PolyIntersector web_mercator_intersector(const double nw[2], const double se[2]) {
+    PolyIntersector r;
+    double nlat, nlng, slat, slng;
+    web_mercator_to_lat_lng(nw, nlat, nlng);
+    web_mercator_to_lat_lng(se, slat, slng);
+    for (int u = 0; u < 2; ++u) {
+        const double h = u ? kWmMaxElevation : kWmMinElevation;
+        r.corners[4 * u + 0] = wgs84_to_ecef(nlat, nlng, h);
+        r.corners[4 * u + 1] = wgs84_to_ecef(nlat, slng, h);
+        r.corners[4 * u + 2] = wgs84_to_ecef(slat, slng, h);
+        r.corners[4 * u + 3] = wgs84_to_ecef(slat, nlng, h);
+    }
+    const V3* c = r.corners;
+    for (int u = 0; u < 2; ++u)
+        for (int i = 0; i < 4; ++i) r.edges[4 * u + i] = unit(v3sub(c[4 * u + (i + 1) % 4], c[4 * u + i]));  // N E S W, down then up
+    for (int i = 0; i < 4; ++i) r.edges[8 + i] = unit(v3sub(c[4 + i], c[i]));                             // NW NE SE SW, upward
+    r.nedges = 12;
+    const V3* e = r.edges;
+    for (int i = 0; i < 4; ++i) r.normals[i] = unit(v3cross(e[i], e[8 + i]));  // N E S W faces
+    r.normals[4] = unit(v3cross(e[1], e[0]));                                  // down
+    r.normals[5] = unit(v3cross(e[5], e[4]));                                  // up
+    r.nnormals = 6;
+    return r;
+}
+
 // Intersector::cache_separating_axes_for_aabb: [own normals, x,y,z, normalize(edge_i x unit_j) if finite], then dedup.
-inline void cache_axes_for_aabb(const PolyIntersector& p, QueryGeom& g) {
+// Axes past kInlineAxes go to `more` (g.more_axes points to it); only a Web Mercator rect has them.
+inline void cache_axes_for_aabb(const PolyIntersector& p, QueryGeom& g, MoreAxes* more = nullptr) {
     V3 all[6 + 3 + 36];
     int n = 0;
     const V3 units[3] = {{1, 0, 0}, {0, 1, 0}, {0, 0, 1}};
@@ -144,17 +297,21 @@ inline void cache_axes_for_aabb(const PolyIntersector& p, QueryGeom& g) {
             if (std::isfinite(c.x) && std::isfinite(c.y) && std::isfinite(c.z)) all[n++] = c;
         }
     g.naxes = 0;
+    g.more_axes = more;
     for (int i = 0; i < n; ++i) {
         bool dupe = false;
         for (int k = 0; k < g.naxes && !dupe; ++k) {
-            const V3 o{g.axes[k][0], g.axes[k][1], g.axes[k][2]};
+            const double* a = geom_axis(g, k);
+            const V3 o{a[0], a[1], a[2]};
             const V3 dm = v3sub(all[i], o), dp = v3add(all[i], o);
             dupe = std::fmin(v3dot(dm, dm), v3dot(dp, dp)) < std::numeric_limits<double>::epsilon();
         }
         if (!dupe) {
-            g.axes[g.naxes][0] = all[i].x;
-            g.axes[g.naxes][1] = all[i].y;
-            g.axes[g.naxes][2] = all[i].z;
+            if (g.naxes >= kInlineAxes && !more) throw std::logic_error("a location with more than kInlineAxes axes and no table for them");
+            double* a = g.naxes < kInlineAxes ? g.axes[g.naxes] : more->a[g.naxes - kInlineAxes];
+            a[0] = all[i].x;
+            a[1] = all[i].y;
+            a[2] = all[i].z;
             ++g.naxes;
         }
     }
@@ -163,9 +320,11 @@ inline void cache_axes_for_aabb(const PolyIntersector& p, QueryGeom& g) {
         g.corners[i][1] = p.corners[i].y;
         g.corners[i][2] = p.corners[i].z;
     }
+    for (int k = kInlineAxes; k < g.naxes; ++k) project_location_axis(g, k, more->proj[k - kInlineAxes][0], more->proj[k - kInlineAxes][1]);
 }
 
-inline QueryGeom make_query_geom(const pcv_location& loc) {
+// `more` holds a Web Mercator rect's axes past kInlineAxes (required for that kind, unused for the others).
+inline QueryGeom make_query_geom(const pcv_location& loc, MoreAxes* more = nullptr) {
     QueryGeom g;
     std::memset(&g, 0, sizeof g);
     g.kind = loc.kind;
@@ -188,6 +347,12 @@ inline QueryGeom make_query_geom(const pcv_location& loc) {
         cache_axes_for_aabb(frustum_intersector(loc.query_from_clip), g);
     } else if (loc.kind == PCV_LOC_OBB) {
         cache_axes_for_aabb(obb_intersector(loc.query_from_obb, loc.half_extent), g);
+    } else if (loc.kind == PCV_LOC_WEB_MERCATOR_RECT) {
+        for (int a = 0; a < 3; ++a) {  // unsorted: a rect that wraps the antimeridian stays wrapped
+            g.aabb_min[a] = loc.aabb_min[a];
+            g.aabb_max[a] = loc.aabb_max[a];
+        }
+        cache_axes_for_aabb(web_mercator_intersector(loc.aabb_min, loc.aabb_max), g, more);
     }
     return g;
 }
@@ -195,16 +360,6 @@ inline QueryGeom make_query_geom(const pcv_location& loc) {
 // The separating-axis test of a location against an arbitrary box [mn, mx] (the point box of an S2 cell, s2_api.inl): sat()
 // of sat.rs:174-194 over the location's cached axes, the box's 8 corners in the Aabb order (x fastest, aabb.rs:114-125), exactly
 // as sat_cube (query.cuh) tests a node cube, whose max is min + edge.  Shared by the device kernels and the test backend.
-// project_location_axis: the location's own projection on axis k (project_location of query.cuh, one axis).
-PCV_GHD void project_location_axis(const QueryGeom& g, int k, double& lo, double& hi) {
-    lo = 1.7976931348623157e308;
-    hi = -1.7976931348623157e308;
-    for (int i = 0; i < 8; ++i) {
-        const double p = g.corners[i][0] * g.axes[k][0] + g.corners[i][1] * g.axes[k][1] + g.corners[i][2] * g.axes[k][2];
-        lo = fmin(lo, p);
-        hi = fmax(hi, p);
-    }
-}
 PCV_GHD void project_box(const double mn[3], const double mx[3], const double ax[3], double& lo, double& hi) {
     lo = 1.7976931348623157e308;
     hi = -1.7976931348623157e308;
@@ -215,13 +370,22 @@ PCV_GHD void project_box(const double mn[3], const double mx[3], const double ax
         hi = fmax(hi, p);
     }
 }
-// kS2RelIn / kS2RelCross / kS2RelOut; aproj[k] = project_location_axis(g, k)
+// kS2RelIn / kS2RelCross / kS2RelOut; aproj[k] = project_location_axis(g, k) for k < kInlineAxes, a Web Mercator rect's table
+// holds the projections on its further axes.  The relation does not depend on the order of the axes.
 PCV_GHD int sat_box(const QueryGeom& g, const double (*aproj)[2], const double mn[3], const double mx[3]) {
     int rel = kS2RelIn;
-    for (int k = 0; k < g.naxes; ++k) {
+    const int ni = g.naxes < kInlineAxes ? g.naxes : kInlineAxes;
+    for (int k = 0; k < ni; ++k) {
         double bmin, bmax;
         project_box(mn, mx, g.axes[k], bmin, bmax);
         const double amin = aproj[k][0], amax = aproj[k][1];
+        if (bmin > amax || bmax < amin) return kS2RelOut;
+        if (amin > bmin || bmax > amax) rel = kS2RelCross;
+    }
+    for (int k = 0; k < g.naxes - kInlineAxes; ++k) {
+        double bmin, bmax;
+        project_box(mn, mx, g.more_axes->a[k], bmin, bmax);
+        const double amin = g.more_axes->proj[k][0], amax = g.more_axes->proj[k][1];
         if (bmin > amax || bmax < amin) return kS2RelOut;
         if (amin > bmin || bmax > amax) rel = kS2RelCross;
     }

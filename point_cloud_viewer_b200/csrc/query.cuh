@@ -48,13 +48,22 @@ __device__ __forceinline__ void project_cube(const double m[3], double e, const 
     }
 }
 
-// sat() of sat.rs:174-194 with A = the location (projections precomputed in aproj) and B = the node cube.
+// sat() of sat.rs:174-194 with A = the location (projections precomputed: in aproj for its inline axes, in its table for a Web
+// Mercator rect's further axes) and B = the node cube.  The relation does not depend on the order of the axes.
 __device__ __forceinline__ uint8_t sat_cube(const QueryGeom& g, const double (*aproj)[2], const double m[3], double e) {
     uint8_t rel = REL_IN;
-    for (int k = 0; k < g.naxes; ++k) {
+    const int ni = min(g.naxes, kInlineAxes);
+    for (int k = 0; k < ni; ++k) {
         double bmin, bmax;
         project_cube(m, e, g.axes[k], bmin, bmax);
         const double amin = aproj[k][0], amax = aproj[k][1];
+        if (bmin > amax || bmax < amin) return REL_OUT;
+        if (amin > bmin || bmax > amax) rel = REL_CROSS;
+    }
+    for (int k = 0; k < g.naxes - kInlineAxes; ++k) {
+        double bmin, bmax;
+        project_cube(m, e, g.more_axes->a[k], bmin, bmax);
+        const double amin = g.more_axes->proj[k][0], amax = g.more_axes->proj[k][1];
         if (bmin > amax || bmax < amin) return REL_OUT;
         if (amin > bmin || bmax > amax) rel = REL_CROSS;
     }
@@ -70,8 +79,10 @@ __device__ __forceinline__ uint8_t node_relation(const QueryGeom& g, const doubl
     return sat_cube(g, aproj, m, e);
 }
 
+// The projections of the location's inline axes (sat_cube projects the others itself).
 __device__ __forceinline__ void project_location(const QueryGeom& g, double (*aproj)[2]) {
-    for (int k = threadIdx.x; k < g.naxes; k += blockDim.x) {
+    const int ni = min(g.naxes, kInlineAxes);
+    for (int k = threadIdx.x; k < ni; k += blockDim.x) {
         double lo = 1.7976931348623157e308, hi = -1.7976931348623157e308;
         for (int i = 0; i < 8; ++i) {
             const double p = g.corners[i][0] * g.axes[k][0] + g.corners[i][1] * g.axes[k][1] + g.corners[i][2] * g.axes[k][2];
@@ -86,7 +97,7 @@ __device__ __forceinline__ void project_location(const QueryGeom& g, double (*ap
 // grid = (ceil(nnodes/256), nloc).  rel[loc * nnodes + node]
 __global__ void __launch_bounds__(256) k_sat_nodes(const QueryGeom* __restrict__ geoms, const QNode* __restrict__ nodes, uint32_t nnodes,
                                                    uint8_t* __restrict__ rel) {
-    __shared__ double aproj[26][2];
+    __shared__ double aproj[kInlineAxes][2];
     const QueryGeom& g = geoms[blockIdx.y];
     project_location(g, aproj);
     __syncthreads();
@@ -120,7 +131,7 @@ __device__ __forceinline__ double num_clamp_d(double x, double lo, double hi) { 
 __global__ void __launch_bounds__(256) k_visible_eval(const QueryGeom* __restrict__ geom, const double* __restrict__ M,
                                                       const QNode* __restrict__ nodes, uint32_t nnodes, uint8_t* __restrict__ rel,
                                                       double* __restrict__ size) {
-    __shared__ double aproj[26][2];
+    __shared__ double aproj[kInlineAxes][2];
     const QueryGeom& g = geom[0];
     project_location(g, aproj);
     __syncthreads();
@@ -235,10 +246,13 @@ __device__ __forceinline__ const uint64_t* stage_cells(const QueryGeom& g, uint6
     return sh;
 }
 
-// PointCulling::contains of the cull kernels: loc_contains, and for a cell union contains_cellid(from_point(p))
-// (s2_cell_union.rs:27-31) on the decoded position, over the union's ids at `cells`.
+// PointCulling::contains of the cull kernels: loc_contains, for a cell union contains_cellid(from_point(p))
+// (s2_cell_union.rs:27-31) on the decoded position, over the union's ids at `cells`, and for a Web Mercator rect its FP64
+// ECEF -> WGS84 -> map test.  Only point queries take these two kinds, so the X-ray kernels' loc_contains does not carry them.
+// Their node (cell) tests never make a tile kTileIn for a rect: its polyhedron is not its point predicate.
 __device__ __forceinline__ bool cull_contains(const QueryGeom& g, const uint64_t* cells, const double p[3]) {
     if (g.kind == kLocCellUnion) return s2_union_contains(cells, g.ncells, s2_cell_id_from_point(p[0], p[1], p[2]));
+    if (g.kind == PCV_LOC_WEB_MERCATOR_RECT) return web_mercator_rect_contains(g.aabb_min, g.aabb_max, p[0], p[1], p[2]);
     return loc_contains(g, p[0], p[1], p[2]);
 }
 
@@ -451,7 +465,7 @@ __global__ void __launch_bounds__(256) k_lod_shuffle(const __grid_constant__ Lod
 // holds points) and hands its existing children to the next level's frontier.  Only visited nodes are ever tested - the
 // all-pairs kernel above (k_sat_nodes) stays for the single-location entry points that need the BFS order.
 struct LocProj {
-    double a[26][2];  // projections of the location's 8 corners on each of its cached axes
+    double a[kInlineAxes][2];  // projections of the location's 8 corners on each of its cached axes
 };
 __global__ void __launch_bounds__(32) k_loc_proj(const QueryGeom* __restrict__ geoms, LocProj* __restrict__ out) {
     project_location(geoms[blockIdx.x], out[blockIdx.x].a);
@@ -593,10 +607,10 @@ struct S2SelectArgs {
     unsigned long long* tested;  // [location]
 };
 __global__ void __launch_bounds__(256) k_s2_select_cells(const __grid_constant__ S2SelectArgs a) {
-    __shared__ double aproj[26][2];
+    __shared__ double aproj[kInlineAxes][2];
     const uint32_t loc = blockIdx.y;
     const QueryGeom& g = a.geoms[loc];
-    for (int k = threadIdx.x; k < 52; k += blockDim.x) aproj[k >> 1][k & 1] = a.proj[loc].a[k >> 1][k & 1];
+    for (int k = threadIdx.x; k < 2 * kInlineAxes; k += blockDim.x) aproj[k >> 1][k & 1] = a.proj[loc].a[k >> 1][k & 1];
     __syncthreads();
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     const int lane = threadIdx.x & 31;

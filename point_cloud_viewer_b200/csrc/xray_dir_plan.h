@@ -93,7 +93,7 @@ inline bool sat_cube_out(const QueryGeom& g, const double m[3], double e) {
     if (g.kind == PCV_LOC_ALL) return false;
     const double mx[3] = {m[0] + e, m[1] + e, m[2] + e};
     for (int k = 0; k < g.naxes; ++k) {
-        const double* ax = g.axes[k];
+        const double* ax = geom_axis(g, k);
         double alo = 1.7976931348623157e308, ahi = -1.7976931348623157e308, blo = alo, bhi = ahi;
         for (int i = 0; i < 8; ++i) {
             const double pa = g.corners[i][0] * ax[0] + g.corners[i][1] * ax[1] + g.corners[i][2] * ax[2];

@@ -6,19 +6,22 @@
   Frustum::new             src/geometry/frustum.rs:101-108
   Frustum::from_matrix4    src/geometry/frustum.rs:111-117
   Obb::new / From<&Aabb> / transformed   src/geometry/obb.rs:19-45
+  WebMercatorRect::from_zoomed_coordinates   src/geometry/web_mercator_rect.rs:40-53 (in the library: pcv_web_mercator_rect)
   Isometry3 (translation + unit quaternion i,j,k,w) algebra as in nalgebra 0.22.
 
 Matrices are numpy (4,4) row/col indexed [r, c]; they are flattened column-major (nalgebra storage)
 when written into a Location.
 """
+import ctypes as C
 import math
 
 import numpy as np
 
+from . import _native as _N
 from ._native import CellUnion as _NativeCellUnion
 from ._native import Location
 
-LOC_ALL, LOC_AABB, LOC_FRUSTUM, LOC_OBB = 0, 1, 2, 3
+LOC_ALL, LOC_AABB, LOC_FRUSTUM, LOC_OBB, LOC_WEB_MERCATOR_RECT = 0, 1, 2, 3, 4
 
 
 # ---- isometries ---------------------------------------------------------------------------------
@@ -164,6 +167,33 @@ def obb(query_from_obb, half_extent):
     loc.obb_from_query[:] = query_from_obb.inverse().as7()
     loc.half_extent[:] = [float(v) for v in half_extent]
     return loc
+
+
+def web_mercator_rect(min_xy, max_xy, z):
+    """WebMercatorRect::from_zoomed_coordinates(min, max, z): the points whose map position at zoom z lies in [min, max), in
+    pixels of the 256 * 2^z map (x east, y south).  x may wrap around the antimeridian (min.x > max.x), which selects nodes but no
+    point.  ValueError where the reference returns None: z > 23, a corner outside [0, 256 * 2^z), max.y < min.y, more than one
+    zoom-0 pixel across, or a non-finite value."""
+    mn = (C.c_double * 2)(*[float(v) for v in min_xy])
+    mx = (C.c_double * 2)(*[float(v) for v in max_xy])
+    loc = Location()
+    try:
+        _N.check(_N.lib().pcv_web_mercator_rect(mn, mx, int(z), C.byref(loc)))
+    except _N.PcvError as e:
+        raise ValueError(str(e)) from None
+    return loc
+
+
+def web_mercator_coord(ecef, z):
+    """WebMercatorCoord::from_lat_lng(ECEF -> WGS84).to_zoomed_coordinate(z): the map position (x, y) of an ECEF point at zoom z,
+    in [0, 256 * 2^z).  ValueError for z > 23."""
+    p = (C.c_double * 3)(*[float(v) for v in ecef])
+    out = (C.c_double * 2)()
+    try:
+        _N.check(_N.lib().pcv_web_mercator_coord(p, int(z), out))
+    except _N.PcvError as e:
+        raise ValueError(str(e)) from None
+    return out[0], out[1]
 
 
 class CellUnion:
