@@ -471,6 +471,34 @@ int pcv_s2_query_cell_unions_batch_device(const pcv_s2cloud* cloud, const pcv_ce
  * octree metas are rejected with the reference's messages). */
 int pcv_s2_write_dir(const pcv_s2cloud* cloud, const char* directory);
 int pcv_s2_load_dir(pcv_ctx* ctx, const char* directory, pcv_s2cloud** out);
+/* S2Splitter::write batch by batch + get_meta (read_write/s2.rs:52-175) for a cloud of any size, straight to a directory in
+ * bounded device memory: the directory is byte for byte what pcv_s2_build + pcv_s2_write_dir write for the same points (for a
+ * PLY file: pcv_s2_build_device over the points pcv_ply_load_device gives), at every budget and split level.
+ *  - Host points (pageable or pinned, SoA or AoS like pcv_s2_build) carry colour / intensity when those pointers are set; a PLY
+ *    file carries the attributes it has.  The total may exceed 2^32 points.
+ *  - max_device_bytes bounds everything the call allocates on the device (0: most of the free memory); a budget that cannot
+ *    hold one minimal batch is PCV_ERR_UNSUPPORTED.  Host memory: two pinned output slots of one batch and 16 B per cell.
+ *  - An existing directory: a cell's files are truncated the first time the call writes them, files of other cells are left
+ *    alone (OpenMode::Truncate).  Its meta.pb is removed before the first cell file is written; the new one is written last,
+ *    through a temporary name, and only on success.  So a failed call (an invalid point in a late batch, an I/O error) leaves
+ *    no loadable directory, where the reference would leave the old meta.pb beside half-rewritten cells.
+ *  - Errors: an invalid ECEF point is pcv_s2_build's PCV_ERR_INVALID for the first one in input order; no points is
+ *    pcv_s2_write_dir's error and writes nothing; a file that cannot be written is PCV_ERR_IO naming it; a truncated PLY body
+ *    is PCV_ERR_IO. */
+typedef struct pcv_s2_dir_build_info {
+    uint64_t num_points, num_cells;
+    uint64_t batches, largest_batch;              /* points per batch                                                  */
+    uint64_t max_device_bytes, peak_device_bytes; /* the budget used; the most the call held at once                   */
+    uint64_t h2d_bytes, d2h_bytes;                /* input read once; cell-ordered output read back once               */
+    uint64_t bytes_written, file_writes;          /* node-file bytes; (cell, batch, attribute) writes                  */
+    double ms_split;                              /* CUDA events around each batch's split, summed over batches        */
+    double ms_input_wait, ms_write_wait, ms_total;/* device time between splits (input); wall time blocked on the
+                                                     writers; wall time of the call                                    */
+} pcv_s2_dir_build_info;
+int pcv_s2_build_to_dir(pcv_ctx* ctx, const pcv_points* host_points, uint32_t split_level, uint64_t max_device_bytes,
+                        const char* dir, pcv_s2_dir_build_info* info /* may be NULL */);
+int pcv_s2_build_from_file_to_dir(pcv_ctx* ctx, const char* ply_path, uint32_t split_level, uint64_t max_device_bytes,
+                                  const char* dir, pcv_s2_dir_build_info* info);
 /* build_xray_quadtree over an S2 cloud (xray/src/build_quadtree.rs with S2 locations), in bounded device memory like
  * pcv_xray_quadtree_bounded[_write_dir]: the same post-order delivery, cancellation, <id>.png + meta[<digits>].pb output and
  * pcv_xray_bounded_info.  The quadtree's frame, rect and levels come from the cloud's box (pcv_s2_info: the exact min and max

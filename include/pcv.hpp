@@ -506,6 +506,20 @@ class S2Cells {
         check(pcv_s2_load_dir(ctx.raw(), directory.c_str(), &s));
         return S2Cells(s);
     }
+    // S2Splitter<RawNodeWriter>::write batch by batch + get_meta, straight to `directory` in bounded device memory: the files
+    // pcv_s2_build + pcv_s2_write_dir would write (pcv_s2_build_to_dir).  Load them with from_directory.
+    static pcv_s2_dir_build_info build_to_directory(Context& ctx, const pcv_points& host_points, const std::string& directory,
+                                                    uint32_t split_level = 20, uint64_t max_device_bytes = 0) {
+        pcv_s2_dir_build_info info{};
+        check(pcv_s2_build_to_dir(ctx.raw(), &host_points, split_level, max_device_bytes, directory.c_str(), &info));
+        return info;
+    }
+    static pcv_s2_dir_build_info build_file_to_directory(Context& ctx, const std::string& ply_path, const std::string& directory,
+                                                         uint32_t split_level = 20, uint64_t max_device_bytes = 0) {
+        pcv_s2_dir_build_info info{};
+        check(pcv_s2_build_from_file_to_dir(ctx.raw(), ply_path.c_str(), split_level, max_device_bytes, directory.c_str(), &info));
+        return info;
+    }
     ~S2Cells() {
         if (s_) pcv_s2_free(s_);
     }

@@ -122,6 +122,26 @@ class Context:
         N.check(N.lib().pcv_s2_load_dir(self.h, os.fsencode(str(directory)), C.byref(out)))
         return S2Cloud(self, out)
 
+    def build_s2_dir(self, directory, x, y, z, rgb=None, intensity=None, split_level=20, max_device_bytes=0, stride=1, n=None):
+        """S2Splitter::write batch by batch + get_meta for host points of any size, straight to `directory`: the files
+        build_s2_cloud(...).write_dir(directory) writes, in at most `max_device_bytes` of device memory (0: most of the free
+        memory).  Returns the pcv_s2_dir_build_info fields as a dict."""
+        if n is None:
+            n = len(x)
+        keep = (x, y, z, rgb, intensity)
+        pts = N.Points(_p(x), _p(y), _p(z), stride, _p(rgb), _p(intensity), int(n))
+        info = N.S2DirBuildInfo()
+        N.check(N.lib().pcv_s2_build_to_dir(self.h, C.byref(pts), int(split_level), int(max_device_bytes), os.fsencode(str(directory)), C.byref(info)))
+        del keep
+        return {f: getattr(info, f) for f, _ in N.S2DirBuildInfo._fields_}
+
+    def build_s2_dir_from_file(self, ply_path, directory, split_level=20, max_device_bytes=0):
+        """build_s2_dir for a PLY file of any size (its colour and intensity when it has them).  Returns the info dict."""
+        info = N.S2DirBuildInfo()
+        N.check(N.lib().pcv_s2_build_from_file_to_dir(self.h, os.fsencode(str(ply_path)), int(split_level), int(max_device_bytes),
+                                                      os.fsencode(str(directory)), C.byref(info)))
+        return {f: getattr(info, f) for f, _ in N.S2DirBuildInfo._fields_}
+
     def s2_union_contains(self, x, y, z, union_ids, stride=1, n=None):
         """CellUnion as PointCulling (geometry/s2_cell_union.rs:27-31): boolean mask over host points."""
         n = int(n if n is not None else len(x))

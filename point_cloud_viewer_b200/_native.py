@@ -185,6 +185,15 @@ class OocInfo(C.Structure):
                 ("ms_top", C.c_double), ("ms_total", C.c_double)]
 
 
+class S2DirBuildInfo(C.Structure):
+    """pcv_s2_dir_build_info (include/pcv.h)."""
+
+    _fields_ = [("num_points", C.c_uint64), ("num_cells", C.c_uint64), ("batches", C.c_uint64), ("largest_batch", C.c_uint64),
+                ("max_device_bytes", C.c_uint64), ("peak_device_bytes", C.c_uint64), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64),
+                ("bytes_written", C.c_uint64), ("file_writes", C.c_uint64), ("ms_split", C.c_double), ("ms_input_wait", C.c_double),
+                ("ms_write_wait", C.c_double), ("ms_total", C.c_double)]
+
+
 # every symbol include/pcv.h declares: (name, restype, argtypes)
 _dp = C.POINTER(C.c_double)
 _u64p = C.POINTER(C.c_uint64)
@@ -272,6 +281,8 @@ SYMBOLS = [
     ("pcv_s2_query_cell_unions_batch_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
     ("pcv_s2_write_dir", C.c_int, [C.c_void_p, C.c_char_p]),
     ("pcv_s2_load_dir", C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),
+    ("pcv_s2_build_to_dir", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_uint32, C.c_uint64, C.c_char_p, C.POINTER(S2DirBuildInfo)]),
+    ("pcv_s2_build_from_file_to_dir", C.c_int, [C.c_void_p, C.c_char_p, C.c_uint32, C.c_uint64, C.c_char_p, C.POINTER(S2DirBuildInfo)]),
     ("pcv_s2_xray_quadtree", C.c_int, [C.c_void_p, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64, XRAY_TILE_FN, C.c_void_p,
                                        C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo)]),
     ("pcv_s2_xray_quadtree_write_dir", C.c_int, [C.c_void_p, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64, C.c_char_p,

@@ -27,6 +27,8 @@
 #include "xray_pyramid.cuh"
 #include "xray_dir_plan.h"
 #include "s2.cuh"
+#include "s2_dir_writer.hpp"
+#include "s2_stream_plan.h"
 #include "synth.cuh"
 
 using namespace pcv;
@@ -578,3 +580,4 @@ int pcv_synth_bbox(int kind, double bbox_min[3], double bbox_max[3], double* res
 #include "shard_api.inl"
 #include "sharded_build.inl"
 #include "ooc_build.inl"
+#include "s2_stream.inl"
