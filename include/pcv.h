@@ -354,6 +354,33 @@ int pcv_xray_quadtree_from_dir_filtered_write_dir(pcv_ctx* ctx, const char* octr
                                                   uint32_t nfilt, uint64_t max_device_bytes, const char* out_dir, pcv_xray_quadtree_info* info_out,
                                                   pcv_xray_bounded_info* bounded_info_out, pcv_xray_dir_info* dir_info_out);
 
+/* The X-ray quadtree straight from one or more S2 directories (meta.pb + cell files, as pcv_s2_write_dir and pcv_s2_build_to_dir
+ * leave them), none of them ever resident as a whole: the same tiles, delivery (every tile after its children; the order across
+ * blocks follows the block level, as in every bounded entry), cancellation, <id>.png + meta<...>.pb outputs and
+ * pcv_xray_bounded_info as pcv_s2_xray_quadtree_clouds over pcv_s2_load_dir of every directory, in the same order.  The
+ * quadtree lies over the union of the directories' meta.pb boxes; XRay tiles are byte for byte the same at every budget; the
+ * attribute strategies (Binning = None) accumulate as the resident path does, so they are equal up to float atomic ordering.
+ * There is no limit on the total, which may exceed device memory and 2^32 points: only one window must fit the budget and hold
+ * fewer than 2^32 points.  One streaming pass over every cell's positions marks the leaves a point falls into and takes every
+ * cell's exact point box; then each block of leaves runs on its window, the cells of any directory whose point box the block's
+ * location (widened by the driver's margin) is not Out of, read from disk (XRay without filters reads .xyz only).  Cells the
+ * previous window holds are copied on the device when the budget has room for both.  max_device_bytes bounds everything the
+ * call allocates, the windows included (0: most of the free device memory).  Host memory holds the cell tables (id, count,
+ * directory, point box: about 64 B per cell), the occupied leaves and the staging of the largest window.  In dir_info_out the
+ * "node" counters count cells.  Errors: ndirs == 0 or a null path -> PCV_ERR_INVALID; an unreadable meta.pb -> PCV_ERR_IO; a
+ * meta.pb that is not a version 12/13 S2 meta, an invalid or duplicated cell id -> PCV_ERR_INVALID; any cell file a meta
+ * declares missing or wrongly sized -> PCV_ERR_NOT_FOUND, found by stat for every directory before the first read (no tile is
+ * delivered); filters and a directory without intensity, or PCV_XRAY_COLORED and a directory without colour -> PCV_ERR_INVALID;
+ * a binned strategy -> PCV_ERR_UNSUPPORTED; a budget too small for the scan pass, a leaf whose window alone does not fit or holds
+ * 2^32 points or more (named), a cell of 2^32 points or more (named by its token) -> PCV_ERR_UNSUPPORTED.  bounded_info_out and
+ * dir_info_out may be NULL. */
+int pcv_s2_xray_quadtree_from_dirs(pcv_ctx* ctx, const char* const* dirs, uint32_t ndirs, const pcv_xray_quadtree_params* params,
+                                   const pcv_interval* filters, uint32_t nfilt, uint64_t max_device_bytes, pcv_xray_tile_fn on_tile, void* user,
+                                   pcv_xray_quadtree_info* info_out, pcv_xray_bounded_info* bounded_info_out, pcv_xray_dir_info* dir_info_out);
+int pcv_s2_xray_quadtree_from_dirs_write_dir(pcv_ctx* ctx, const char* const* dirs, uint32_t ndirs, const pcv_xray_quadtree_params* params,
+                                             const pcv_interval* filters, uint32_t nfilt, uint64_t max_device_bytes, const char* out_dir,
+                                             pcv_xray_quadtree_info* info_out, pcv_xray_bounded_info* bounded_info_out, pcv_xray_dir_info* dir_info_out);
+
 /* The X-ray quadtree of several resident octrees at once (build_xray_quadtree over a list of point_cloud_locations,
  * point_cloud_client/src/lib.rs:118-141), with filter intervals on the intensity.  The quadtree lies over the union of the
  * clouds' boxes (component-wise min and max, empty clouds included).  A leaf is made of every point of every cloud that its

@@ -215,6 +215,28 @@ class Context:
         return _xray_call(N.lib().pcv_xray_quadtree_from_dir_filtered_write_dir,
                           (self.h, os.fsencode(str(octree_dir)), C.byref(pr), _p(f), nf, int(max_device_bytes), os.fsencode(str(out_dir))), True)
 
+    # -- X-ray quadtrees straight from S2 directories (never resident as a whole)
+    def xray_quadtree_from_s2_dirs(self, dirs, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0, query_from_global=None,
+                                   background=(255, 255, 255, 255), root=(0, 0), on_tile=None, keep_tiles=True, max_device_bytes=0, filter_intervals=()):
+        """xray_quadtree_clouds over load_s2_dir of every directory in `dirs` (one path or a list of paths), streamed from disk
+        window by window: the same (info dict, tiles) and keywords, in any total size.  `max_device_bytes` bounds everything the
+        call allocates (0: most of the free memory); the info dict also holds the pcv_xray_dir_info fields (its node counters
+        count cells)."""
+        pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
+        f, nf = _intervals(filter_intervals)
+        arr, keep = _dir_list(dirs)
+        return _xray_call(N.lib().pcv_s2_xray_quadtree_from_dirs, (self.h, arr, len(keep), C.byref(pr), _p(f), nf, int(max_device_bytes)), True, True, on_tile,
+                          keep_tiles)
+
+    def xray_quadtree_from_s2_dirs_write_dir(self, dirs, out_dir, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0,
+                                             query_from_global=None, background=(255, 255, 255, 255), root=(0, 0), max_device_bytes=0, filter_intervals=()):
+        """xray_quadtree_from_s2_dirs with the reference's outputs: <out_dir>/<node id>.png + the quadtree's meta file."""
+        pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
+        f, nf = _intervals(filter_intervals)
+        arr, keep = _dir_list(dirs)
+        return _xray_call(N.lib().pcv_s2_xray_quadtree_from_dirs_write_dir,
+                          (self.h, arr, len(keep), C.byref(pr), _p(f), nf, int(max_device_bytes), os.fsencode(str(out_dir))), True)
+
     # -- X-ray quadtrees over several resident clouds at once
     def xray_quadtree_clouds(self, clouds, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0, query_from_global=None,
                              background=(255, 255, 255, 255), root=(0, 0), on_tile=None, keep_tiles=True, filter_intervals=(), max_device_bytes=0):
@@ -971,6 +993,14 @@ def _cloud_handles(clouds):
     else:
         raise TypeError("clouds must all be Octree or all be S2Cloud")
     return octrees, (C.c_void_p * len(clouds))(*[c.h for c in clouds])
+
+
+def _dir_list(dirs):
+    """One path or a list of paths -> (char* array, the encoded paths it points into)."""
+    if isinstance(dirs, (str, bytes, os.PathLike)):
+        dirs = [dirs]
+    keep = [os.fsencode(str(d) if not isinstance(d, bytes) else d) for d in dirs]
+    return (C.c_char_p * max(1, len(keep)))(*keep), keep
 
 
 def _xray_call(fn, args, dir_info, with_tiles=False, on_tile=None, keep_tiles=True):

@@ -291,6 +291,11 @@ SYMBOLS = [
                                               C.c_void_p, C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo)]),
     ("pcv_s2_xray_quadtree_clouds_write_dir", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64,
                                                         C.c_char_p, C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo)]),
+    ("pcv_s2_xray_quadtree_from_dirs", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64,
+                                                 XRAY_TILE_FN, C.c_void_p, C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo), C.POINTER(XrayDirInfo)]),
+    ("pcv_s2_xray_quadtree_from_dirs_write_dir", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32,
+                                                           C.c_uint64, C.c_char_p, C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo),
+                                                           C.POINTER(XrayDirInfo)]),
     ("pcv_s2_union_contains", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_void_p, C.c_uint32, C.c_void_p]),
     ("pcv_prefix_histogram_device", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_double, _dp, _dp, C.c_uint32, C.c_void_p]),
     ("pcv_prefix_histogram_bbox_device", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_double, _dp, _dp, C.c_uint32, C.c_void_p, _dp, _dp]),

@@ -1050,6 +1050,59 @@ __global__ void __launch_bounds__(256) k_xray_occupy_cells(const __grid_constant
         }
     }
 }
+// The scan pass of the X-ray quadtree built from S2 directories (s2_dir_xray.inl): one chunk of cell pieces (a cell larger
+// than a chunk is cut across chunks) streamed through the device, every position read once for two things: (a) the leaves it
+// falls into, marked into the set as k_xray_occupy_cells marks them, and (b) the point box of its cell, reduced over
+// f64_order_key as k_s2_cell_boxes reduces it (warp shuffles, then one atomic per warp and bound) into the slot of the cell's
+// index in the directory-wide table.  Min and max do not depend on how cells are cut or in which order tiles meet, so the box
+// is the one s2_location_tables computes for the loaded cloud, bit for bit.  Running a chunk again is idempotent.
+struct S2DirScanArgs {
+    XrayOccupyCellsArgs occ;   // nodes: the chunk's pieces as Float64 nodes (m = -0.0, e = 1); tiles: their work tiles
+    const uint32_t* cell;      // [piece] its cell in the directory-wide table
+    unsigned long long* kmin;  // [cell * 3 + axis], preset to ~0 / 0
+    unsigned long long* kmax;
+};
+__global__ void __launch_bounds__(256) k_s2_dir_scan(const __grid_constant__ S2DirScanArgs s) {
+    const XrayOccupyCellsArgs& a = s.occ;
+    const uint64_t cells = 1ull << a.level;
+    for (uint32_t ti = blockIdx.x; ti < a.ntiles; ti += gridDim.x) {
+        const QTile t = a.tiles[ti];
+        const QNode nd = a.nodes[t.node];
+        unsigned long long lo[3] = {~0ull, ~0ull, ~0ull}, hi[3] = {0ull, 0ull, 0ull};
+        for (uint32_t i = threadIdx.x; i < t.count; i += blockDim.x) {
+            double p[3];
+            decode_point(a.xyz, nd, 8, t.first + i, p);  // Float64 node: the stored doubles, bit for bit
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                const unsigned long long key = f64_order_key(p[k]);
+                lo[k] = min(lo[k], key);
+                hi[k] = max(hi[k], key);
+            }
+            int64_t x0, x1, y0, y1;
+            xray_point_cells(p, a.has_q ? a.query_from_global : nullptr, a.x0, a.y0, a.edge, a.margin, cells, x0, x1, y0, y1);
+            for (int64_t ix = x0; ix <= x1; ++ix)
+                for (int64_t iy = y0; iy <= y1; ++iy) {
+                    const uint64_t idx = xray_quad_index((uint64_t)ix, (uint64_t)iy, a.level);
+                    if (idx >= a.lo && idx <= a.hi) occupy_insert(a, idx);
+                }
+        }
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                lo[k] = min(lo[k], __shfl_xor_sync(0xffffffffu, lo[k], o));
+                hi[k] = max(hi[k], __shfl_xor_sync(0xffffffffu, hi[k], o));
+            }
+        if ((threadIdx.x & 31) == 0 && threadIdx.x < t.count) {
+            const size_t c = s.cell[t.node];
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                atomicMin(&s.kmin[3 * c + k], lo[k]);
+                atomicMax(&s.kmax[3 * c + k], hi[k]);
+            }
+        }
+    }
+}
 struct XraySubArgs {
     const uint32_t* sub_off;    // [nleaf * nsub + 1] exclusive offsets into keys
     const uint32_t* keys;

@@ -148,4 +148,43 @@ inline std::string decode_s2_meta(const std::string& buf, S2MetaData& m, int& ve
     return "";
 }
 
+// The cells of an S2 directory as pcv_s2_load_dir lays them out, from its meta.pb alone: cells in id order, the first slot
+// of each, the total and the deepest cell level (the split level).
+struct S2DirCells {
+    S2MetaData m;                // the box and attributes; m.ids / m.counts in the proto's order
+    std::vector<uint64_t> ids, counts, starts;
+    uint64_t n = 0;
+    int level = -1;
+};
+// meta.pb of `dir` -> its cells.  PCV_OK, or PCV_ERR_IO (meta.pb unreadable) / PCV_ERR_INVALID (not an S2 meta of version
+// 12 or 13, an invalid or duplicated cell id) with the message in `err`.  No cell file is touched.
+inline int open_s2_dir_cells(const std::string& dir, S2DirCells& out, std::string& err) {
+    const std::string base = dir + "/";
+    std::string raw;
+    out = S2DirCells{};
+    if (!read_whole_file(base + "meta.pb", raw)) return err = "cannot read " + base + "meta.pb", PCV_ERR_IO;
+    int version = 0;
+    err = decode_s2_meta(raw, out.m, version);
+    if (!err.empty()) return PCV_ERR_INVALID;
+    // cells in id order (the proto carries them in hash-map order)
+    const S2MetaData& m = out.m;
+    std::vector<size_t> order(m.ids.size());
+    for (size_t k = 0; k < order.size(); ++k) order[k] = k;
+    std::sort(order.begin(), order.end(), [&](size_t a, size_t b) { return m.ids[a] < m.ids[b]; });
+    for (size_t k : order) {
+        char buf[96];
+        if (!s2_is_valid(m.ids[k])) {
+            snprintf(buf, sizeof buf, "invalid S2 cell id %llx in meta.pb", (unsigned long long)m.ids[k]);
+            return err = buf, PCV_ERR_INVALID;
+        }
+        if (!out.ids.empty() && out.ids.back() == m.ids[k]) return err = "cell " + s2_to_token(m.ids[k]) + " is listed twice", PCV_ERR_INVALID;
+        out.ids.push_back(m.ids[k]);
+        out.counts.push_back(m.counts[k]);
+        out.starts.push_back(out.n);
+        out.n += m.counts[k];
+        out.level = std::max(out.level, s2_level(m.ids[k]));
+    }
+    return PCV_OK;
+}
+
 }  // namespace pcv

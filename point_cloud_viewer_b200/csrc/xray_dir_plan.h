@@ -157,16 +157,20 @@ inline pcv_location xray_block_location(const QuadRect& rect, int B, uint64_t bi
     return xray_location(tmin, tmax, qfg);
 }
 
-// Block depth g of the directory driver: the largest g <= g_max for which the block images, the node selection and the
-// largest window over the occupied blocks at level deepest - g (`window_max(g)`, UINT64_MAX: a window too large to hold) fit
-// the budget besides `fixed`.  A smaller g means a deeper block level and smaller windows.  -1: not even g = 0 fits.
-inline int xray_dir_block_depth(uint64_t budget, uint64_t fixed, int depth, int g_max, uint64_t leaf_bytes, uint64_t tile_bytes, uint64_t per_loc,
-                                const std::function<uint64_t(int)>& window_max) {
+// Block depth g of a directory driver: the largest g <= g_max whose plan `fits(g, w)` holds the block images, the leaf
+// producer's working set and the largest window over the occupied blocks at level deepest - g (`window_max(g)`, UINT64_MAX:
+// a window too large to hold).  A smaller g means a deeper block level and smaller windows.  -1: not even g = 0 fits.
+inline int xray_dir_block_depth(int g_max, const std::function<uint64_t(int)>& window_max, const std::function<bool(int, uint64_t)>& fits) {
     for (int g = g_max; g >= 0; --g) {
         const uint64_t w = window_max(g);
-        if (w != UINT64_MAX && xray_octree_plan(budget, fixed, w, depth, g, per_loc, leaf_bytes, tile_bytes).g == g) return g;
+        if (w != UINT64_MAX && fits(g, w)) return g;
     }
     return -1;
+}
+// ... for the octree directory: the block images, the node selection and the window fit the budget besides `fixed`.
+inline int xray_dir_block_depth(uint64_t budget, uint64_t fixed, int depth, int g_max, uint64_t leaf_bytes, uint64_t tile_bytes, uint64_t per_loc,
+                                const std::function<uint64_t(int)>& window_max) {
+    return xray_dir_block_depth(g_max, window_max, [&](int g, uint64_t w) { return xray_octree_plan(budget, fixed, w, depth, g, per_loc, leaf_bytes, tile_bytes).g == g; });
 }
 
 }  // namespace pcv
