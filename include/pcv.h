@@ -554,6 +554,51 @@ int pcv_s2_xray_quadtree_clouds(const pcv_s2cloud* const* clouds, uint32_t n, co
 int pcv_s2_xray_quadtree_clouds_write_dir(const pcv_s2cloud* const* clouds, uint32_t n, const pcv_xray_quadtree_params* params, const pcv_interval* filters,
                                           uint32_t nfilt, uint64_t max_device_bytes, const char* directory, pcv_xray_quadtree_info* info_out,
                                           pcv_xray_bounded_info* bounded_info_out);
+/* ---- point queries straight from an S2 directory (S2Cells over OnDiskDataProvider, s2_cells/mod.rs:203-216) ---- */
+/* A directory-backed S2 cloud.  Every call returns what the same call returns over pcv_s2_load_dir of the directory: the same cell
+ * lists in id order; the same batches (sizes, and element for element xyz, rgb - NULL for a directory without colour -,
+ * intensity and src_index, the slot: the cell's start + j, as load_dir reports it); for the batch calls the same counts and
+ * tested.  Unlike load_dir the total has no limit: it may exceed device memory and 2^32 points (src_index keeps counting in u64).
+ *  - open reads meta.pb and stats every cell file the meta declares; it reads no cell data.  Its errors are those of
+ *    pcv_s2_load_dir and pcv_s2_xray_quadtree_from_dirs: meta.pb unreadable -> PCV_ERR_IO; not an S2 meta of version 12 / 13, an
+ *    invalid or repeated cell id -> PCV_ERR_INVALID; a declared file missing or of the wrong size -> PCV_ERR_NOT_FOUND; a cell
+ *    of 2^32 points or more -> PCV_ERR_UNSUPPORTED naming its token; a budget that cannot hold the handle's tables, the
+ *    selection of one location and one chunk -> PCV_ERR_UNSUPPORTED.  A file that shrinks after open is PCV_ERR_NOT_FOUND from
+ *    the call that reads it.
+ *  - max_device_bytes (0: most of the free memory) bounds everything the handle and its calls allocate: the cell table reserved
+ *    at open (a Float64 query node, the id and the 48 B point box per cell), the selection scratch, the locations' tables and
+ *    the chunks.  pcv_s2_dir_last_stats: peak_device_bytes <= max_device_bytes after every call.
+ *  - Selection: cell unions and AllPoints select by id range and read no file.  Aabb, Obb, Frustum and WebMercatorRect select by
+ *    each cell's exact point box (as pcv_s2_cells_in_location); the boxes need every position, so the first call that needs them
+ *    streams every .xyz file once and keeps the boxes on the handle (that call's bytes_read, node_files_read and ms_select
+ *    include the scan; no later call repeats it).  The boxes equal the loaded cloud's bit for bit.
+ *  - Reading: a query reads only the selected cells that hold points, in chunks cut at 2048-point tile boundaries (a cell
+ *    larger than a chunk is read in byte ranges across consecutive chunks); host threads read chunk i+1 while the device culls
+ *    chunk i.  pcv_s2_dir_query_points / _query_cell_union read .xyz, .rgb when the directory has colour and .intensity when it
+ *    has intensity; the batch calls read .xyz, and .intensity only with filters.  A batch call reads every cell some location
+ *    selects once, each (location, cell) pair getting its own work tiles; a batch whose tables, selection and one chunk do not
+ *    fit the budget -> PCV_ERR_UNSUPPORTED ("split the batch").
+ *  - Filters on a directory without intensity -> PCV_ERR_INVALID; a callback that stops -> PCV_ERR_CANCELLED.  The stats'
+ *    "node" counters count cells.  A handle serialises on its context. */
+typedef struct pcv_s2_dir pcv_s2_dir;
+int pcv_s2_dir_open(pcv_ctx* ctx, const char* dir, uint64_t max_device_bytes, pcv_s2_dir** out);
+void pcv_s2_dir_close(pcv_s2_dir* d);
+int pcv_s2_dir_info(const pcv_s2_dir* d, uint64_t* num_cells, uint64_t* num_points, uint32_t* split_level, double bbox_min[3], double bbox_max[3],
+                    int* has_color, int* has_intensity);                                            /* == pcv_s2_info of load_dir */
+int pcv_s2_dir_cells(const pcv_s2_dir* d, uint64_t* ids_out, uint64_t* num_points_out);            /* == pcv_s2_cells            */
+int pcv_s2_dir_cell_data(const pcv_s2_dir* d, uint64_t cell_id, double* xyz_out, uint8_t* rgb_out, float* intensity_out,
+                         uint64_t* src_index_out);                                                   /* points_in_node, from the files */
+int pcv_s2_dir_cells_in_union(const pcv_s2_dir* d, const uint64_t* union_ids, uint32_t n_union, uint64_t* ids_out, uint64_t cap, uint64_t* n_out);
+int pcv_s2_dir_cells_in_location(const pcv_s2_dir* d, const pcv_location* loc, uint64_t* ids_out, uint64_t cap, uint64_t* n_out);
+int pcv_s2_dir_query_points(const pcv_s2_dir* d, const pcv_location* loc, const pcv_interval* filters, uint32_t nfilt, uint64_t batch_size,
+                            pcv_batch_cb cb, void* user);
+int pcv_s2_dir_query_cell_union(const pcv_s2_dir* d, const pcv_cell_union* cu, const pcv_interval* filters, uint32_t nfilt, uint64_t batch_size,
+                                pcv_batch_cb cb, void* user);
+int pcv_s2_dir_query_batch(const pcv_s2_dir* d, const pcv_location* locs, uint32_t nloc, const pcv_interval* filters, uint32_t nfilt,
+                           uint64_t* counts_out, uint64_t* tested_out);
+int pcv_s2_dir_query_cell_unions_batch(const pcv_s2_dir* d, const pcv_cell_union* unions, uint32_t nunion, const pcv_interval* filters,
+                                       uint32_t nfilt, uint64_t* counts_out, uint64_t* tested_out);
+int pcv_s2_dir_last_stats(const pcv_s2_dir* d, pcv_dir_query_stats* out);
 /* CellUnion::contains for arbitrary points: mask_out[i] = union.contains_cellid(CellID::from_point(p_i)). */
 int pcv_s2_union_contains(pcv_ctx* ctx, const pcv_points* host_points, const uint64_t* union_ids, uint32_t n_union, uint8_t* mask_out);
 

@@ -637,6 +637,71 @@ class S2Cells {
     pcv_s2cloud* s_;
 };
 
+// S2Cells over an OnDiskDataProvider (mod.rs:203-216): the directory queried where it lies (pcv_s2_dir).  Every call reads only
+// the cells it selects, within `max_device_bytes`, and returns what S2Cells::from_directory's does (source_index = slot).
+class S2CellsDir {
+   public:
+    S2CellsDir(Context& ctx, const std::string& dir, uint64_t max_device_bytes = 0) { check(pcv_s2_dir_open(ctx.raw(), dir.c_str(), max_device_bytes, &d_)); }
+    S2CellsDir(const S2CellsDir&) = delete;
+    S2CellsDir& operator=(const S2CellsDir&) = delete;
+    ~S2CellsDir() { pcv_s2_dir_close(d_); }
+    // AllPoints (nullptr) / S2Cells(cell_union): the cells whose id range intersects it, no file read
+    std::vector<CellID> nodes_in_location(const CellUnion* cell_union) const {
+        uint64_t n = 0;
+        const uint64_t* u = cell_union ? cell_union->data() : nullptr;
+        const uint32_t nu = cell_union ? (uint32_t)cell_union->size() : 0;
+        check(pcv_s2_dir_cells_in_union(d_, u, nu, nullptr, 0, &n));
+        std::vector<CellID> out(n);
+        check(pcv_s2_dir_cells_in_union(d_, u, nu, out.data(), n, &n));
+        return out;
+    }
+    // S2Cells::nodes_in_location over the directory (the first polyhedral call reads every position once for the point boxes)
+    std::vector<CellID> nodes_in_location(const PointLocation& loc) const {
+        uint64_t n = 0;
+        check(pcv_s2_dir_cells_in_location(d_, &loc.raw, nullptr, 0, &n));
+        std::vector<CellID> out(n);
+        check(pcv_s2_dir_cells_in_location(d_, &loc.raw, out.data(), n, &n));
+        return out;
+    }
+    bool for_each_batch(const PointQuery& query, size_t batch_size, const std::function<bool(PointsBatch&&)>& func) const {
+        const std::vector<pcv_interval> f = detail::raw_intervals(query.filter_intervals);
+        return detail::stream_batches(func, [&](pcv_batch_cb cb, void* user) {
+            return pcv_s2_dir_query_points(d_, &query.location.raw, f.empty() ? nullptr : f.data(), (uint32_t)f.size(), batch_size, cb, user);
+        });
+    }
+    bool for_each_batch(const CellUnion& cell_union, const std::vector<ClosedInterval>& filter_intervals, size_t batch_size,
+                        const std::function<bool(PointsBatch&&)>& func) const {
+        const pcv_cell_union cu = detail::raw_union(cell_union);
+        const std::vector<pcv_interval> f = detail::raw_intervals(filter_intervals);
+        return detail::stream_batches(func, [&](pcv_batch_cb cb, void* user) {
+            return pcv_s2_dir_query_cell_union(d_, &cu, f.empty() ? nullptr : f.data(), (uint32_t)f.size(), batch_size, cb, user);
+        });
+    }
+    // survivors and tested points of every location / cell union, each selected cell read once
+    void query_batch(const std::vector<PointLocation>& locs, std::vector<uint64_t>& counts, std::vector<uint64_t>& tested) const {
+        std::vector<pcv_location> raw;
+        for (auto& l : locs) raw.push_back(l.raw);
+        counts.assign(locs.size(), 0);
+        tested.assign(locs.size(), 0);
+        check(pcv_s2_dir_query_batch(d_, raw.data(), (uint32_t)raw.size(), nullptr, 0, counts.data(), tested.data()));
+    }
+    void query_batch(const std::vector<CellUnion>& unions, std::vector<uint64_t>& counts, std::vector<uint64_t>& tested) const {
+        const std::vector<pcv_cell_union> raw = detail::raw_unions(unions);
+        counts.assign(unions.size(), 0);
+        tested.assign(unions.size(), 0);
+        check(pcv_s2_dir_query_cell_unions_batch(d_, raw.data(), (uint32_t)raw.size(), nullptr, 0, counts.data(), tested.data()));
+    }
+    pcv_dir_query_stats last_stats() const {
+        pcv_dir_query_stats st{};
+        check(pcv_s2_dir_last_stats(d_, &st));
+        return st;
+    }
+    pcv_s2_dir* raw() const { return d_; }
+
+   private:
+    pcv_s2_dir* d_ = nullptr;
+};
+
 // build_xray_quadtree over several resident octrees at once (point_cloud_client/src/lib.rs:118-141): the quadtree over the union
 // of their boxes, every leaf made of the points of all of them that its location contains and that pass `filter_intervals`.
 // Tiles through `on_tile` in post-order, as Octree::build_xray_quadtree delivers them (pcv_xray_quadtree_clouds).

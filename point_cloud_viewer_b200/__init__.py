@@ -122,6 +122,10 @@ class Context:
         N.check(N.lib().pcv_s2_load_dir(self.h, os.fsencode(str(directory)), C.byref(out)))
         return S2Cloud(self, out)
 
+    def open_s2_dir(self, directory, max_device_bytes=0):
+        """An S2Dir over the S2 directory `directory`: queries read only the cells they select (0: most of the free memory)."""
+        return S2Dir(self, directory, max_device_bytes)
+
     def build_s2_dir(self, directory, x, y, z, rgb=None, intensity=None, split_level=20, max_device_bytes=0, stride=1, n=None):
         """S2Splitter::write batch by batch + get_meta for host points of any size, straight to `directory`: the files
         build_s2_cloud(...).write_dir(directory) writes, in at most `max_device_bytes` of device memory (0: most of the free
@@ -943,6 +947,84 @@ class S2Cloud:
         pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
         f, nf = _intervals(filter_intervals)
         return _xray_call(N.lib().pcv_s2_xray_quadtree_write_dir, (self.h, C.byref(pr), _p(f), nf, int(max_device_bytes), os.fsencode(str(directory))), False)
+
+
+class S2Dir:
+    """An S2 directory queried where it lies (pcv_s2_dir): the cell table is on the device, and every query reads, uploads and
+    culls only the cells it selects, in chunks, within `max_device_bytes`.  Attributes and methods have the shapes of S2Cloud's
+    (query_batch returns (counts, tested) like S2Cloud.query_batch_device); every result equals S2Cloud's over load_s2_dir of
+    the directory, `src` being the slot.  The first polyhedral query reads every position once for the cells' point boxes."""
+
+    def __init__(self, ctx, directory, max_device_bytes=0):
+        self.ctx = ctx
+        self.h = None
+        h = C.c_void_p()
+        N.check(N.lib().pcv_s2_dir_open(ctx.h, os.fsencode(str(directory)), int(max_device_bytes), C.byref(h)))
+        self.h = h
+        nc, npnt, lvl = C.c_uint64(), C.c_uint64(), C.c_uint32()
+        mn, mx = (C.c_double * 3)(), (C.c_double * 3)()
+        hc, hi = C.c_int(), C.c_int()
+        N.check(N.lib().pcv_s2_dir_info(self.h, C.byref(nc), C.byref(npnt), C.byref(lvl), mn, mx, C.byref(hc), C.byref(hi)))
+        self.num_cells, self.num_points, self.split_level = nc.value, npnt.value, lvl.value
+        self.bbox_min, self.bbox_max = np.array(mn), np.array(mx)
+        self.has_color, self.has_intensity = bool(hc.value), bool(hi.value)
+        self.cell_ids = np.zeros(self.num_cells, np.uint64)
+        self.cell_counts = np.zeros(self.num_cells, np.uint64)
+        N.check(N.lib().pcv_s2_dir_cells(self.h, _p(self.cell_ids), _p(self.cell_counts)))
+
+    def close(self):
+        if self.h and self.ctx.h:
+            N.lib().pcv_s2_dir_close(self.h)
+        self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def cell_data(self, cell_id):
+        """points_in_node from the cell's files: (xyz f64 (n, 3), rgb or None, intensity or None, slot)."""
+        k = int(np.searchsorted(self.cell_ids, np.uint64(cell_id)))
+        n = int(self.cell_counts[k]) if k < self.num_cells and int(self.cell_ids[k]) == int(cell_id) else 0
+        xyz = np.zeros((n, 3), np.float64)
+        rgb = np.zeros((n, 3), np.uint8) if self.has_color else None
+        inten = np.zeros(n, np.float32) if self.has_intensity else None
+        src = np.zeros(n, np.uint64)
+        N.check(N.lib().pcv_s2_dir_cell_data(self.h, int(cell_id), _p(xyz), _p(rgb), _p(inten), _p(src)))
+        return xyz, rgb, inten, src
+
+    def cells_in_union(self, union_ids=None):
+        """nodes_in_location for AllPoints (None) / S2Cells(CellUnion); no file is read."""
+        u = None if union_ids is None else np.ascontiguousarray(union_ids, np.uint64)
+        out = np.zeros(self.num_cells, np.uint64)
+        n = C.c_uint64()
+        N.check(N.lib().pcv_s2_dir_cells_in_union(self.h, _p(u), 0 if u is None else len(u), _p(out), len(out), C.byref(n)))
+        return out[: n.value]
+
+    def cells_in_location(self, loc):
+        """S2Cloud.cells_in_location over the directory: a pcv_location or a geometry.CellUnion."""
+        if isinstance(loc, geometry.CellUnion):  # an empty union selects no cell (None would mean AllPoints)
+            return self.cells_in_union(loc.ids) if len(loc.ids) else np.zeros(0, np.uint64)
+        out = np.zeros(max(self.num_cells, 1), np.uint64)
+        n = C.c_uint64()
+        N.check(N.lib().pcv_s2_dir_cells_in_location(self.h, C.byref(loc), _p(out), self.num_cells, C.byref(n)))
+        return out[: n.value]
+
+    def query_points(self, loc, callback=None, filters=(), batch_size=500000):
+        """S2Cloud.query_points over the directory; `src` holds every point's slot."""
+        fn = N.lib().pcv_s2_dir_query_cell_union if isinstance(loc, geometry.CellUnion) else N.lib().pcv_s2_dir_query_points
+        return _query_points(fn, self.h, loc, callback, filters, batch_size)
+
+    def query_batch(self, locs, filters=()):
+        """(counts, tested) of S2Cloud.query_batch_device, every selected cell read once."""
+        return _query_batch(N.lib().pcv_s2_dir_query_batch, N.lib().pcv_s2_dir_query_cell_unions_batch, self.h, locs, filters)
+
+    def last_stats(self):
+        """pcv_dir_query_stats of the last call on the handle ("node" counters count cells)."""
+        st = N.DirQueryStats()
+        N.check(N.lib().pcv_s2_dir_last_stats(self.h, C.byref(st)))
+        return {k: getattr(st, k) for k, _ in N.DirQueryStats._fields_}
 
 
 def s2_token(cell_id):

@@ -281,6 +281,18 @@ SYMBOLS = [
     ("pcv_s2_query_cell_unions_batch_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
     ("pcv_s2_write_dir", C.c_int, [C.c_void_p, C.c_char_p]),
     ("pcv_s2_load_dir", C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),
+    ("pcv_s2_dir_open", C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, C.POINTER(C.c_void_p)]),
+    ("pcv_s2_dir_close", None, [C.c_void_p]),
+    ("pcv_s2_dir_info", C.c_int, [C.c_void_p, _u64p, _u64p, C.POINTER(C.c_uint32), _dp, _dp, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    ("pcv_s2_dir_cells", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("pcv_s2_dir_cell_data", C.c_int, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("pcv_s2_dir_cells_in_union", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, _u64p]),
+    ("pcv_s2_dir_cells_in_location", C.c_int, [C.c_void_p, C.POINTER(Location), C.c_void_p, C.c_uint64, _u64p]),
+    ("pcv_s2_dir_query_points", C.c_int, [C.c_void_p, C.POINTER(Location), C.c_void_p, C.c_uint32, C.c_uint64, BATCH_CB, C.c_void_p]),
+    ("pcv_s2_dir_query_cell_union", C.c_int, [C.c_void_p, C.POINTER(CellUnion), C.c_void_p, C.c_uint32, C.c_uint64, BATCH_CB, C.c_void_p]),
+    ("pcv_s2_dir_query_batch", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
+    ("pcv_s2_dir_query_cell_unions_batch", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
+    ("pcv_s2_dir_last_stats", C.c_int, [C.c_void_p, C.POINTER(DirQueryStats)]),
     ("pcv_s2_build_to_dir", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_uint32, C.c_uint64, C.c_char_p, C.POINTER(S2DirBuildInfo)]),
     ("pcv_s2_build_from_file_to_dir", C.c_int, [C.c_void_p, C.c_char_p, C.c_uint32, C.c_uint64, C.c_char_p, C.POINTER(S2DirBuildInfo)]),
     ("pcv_s2_xray_quadtree", C.c_int, [C.c_void_p, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64, XRAY_TILE_FN, C.c_void_p,

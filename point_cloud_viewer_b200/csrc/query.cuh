@@ -363,14 +363,15 @@ __global__ void __launch_bounds__(256) k_cull(const __grid_constant__ CullArgs a
     cull_tile<WRITE, false, RGB>(a, nullptr, nullptr);
 }
 // One chunk of a directory-backed query: `nodes` / `tiles` are the chunk's pieces (chunk-local offsets), `src` / `out_src` unused.
+// RGB = false: an S2 directory without colour.
 struct CullChunkArgs {
     CullArgs c;
-    const uint64_t* slot_base;  // [piece] point_offset of the piece's node + the piece's first point
+    const uint64_t* slot_base;  // [piece] the slot of the piece's first point (octree: point_offset + first; S2 cell: start + first)
     uint64_t* out_slot;
 };
-template <bool WRITE>
+template <bool WRITE, bool RGB = true>
 __global__ void __launch_bounds__(256) k_cull_chunk(const __grid_constant__ CullChunkArgs a) {
-    cull_tile<WRITE, true>(a.c, a.slot_base, a.out_slot);
+    cull_tile<WRITE, true, RGB>(a.c, a.slot_base, a.out_slot);
 }
 
 // Exclusive scan of n u32 values in place; total (u64) to *total_out.  Single block; n is at most a few million tiles.
@@ -1055,13 +1056,15 @@ __global__ void __launch_bounds__(256) k_xray_occupy_cells(const __grid_constant
 // falls into, marked into the set as k_xray_occupy_cells marks them, and (b) the point box of its cell, reduced over
 // f64_order_key as k_s2_cell_boxes reduces it (warp shuffles, then one atomic per warp and bound) into the slot of the cell's
 // index in the directory-wide table.  Min and max do not depend on how cells are cut or in which order tiles meet, so the box
-// is the one s2_location_tables computes for the loaded cloud, bit for bit.  Running a chunk again is idempotent.
+// is the one s2_location_tables computes for the loaded cloud, bit for bit.  Running a chunk again is idempotent.  MARK = false
+// reduces the boxes only (the S2 directory handle, s2_dir_query.inl): the set and the leaf arguments of `occ` are unused.
 struct S2DirScanArgs {
     XrayOccupyCellsArgs occ;   // nodes: the chunk's pieces as Float64 nodes (m = -0.0, e = 1); tiles: their work tiles
     const uint32_t* cell;      // [piece] its cell in the directory-wide table
     unsigned long long* kmin;  // [cell * 3 + axis], preset to ~0 / 0
     unsigned long long* kmax;
 };
+template <bool MARK>
 __global__ void __launch_bounds__(256) k_s2_dir_scan(const __grid_constant__ S2DirScanArgs s) {
     const XrayOccupyCellsArgs& a = s.occ;
     const uint64_t cells = 1ull << a.level;
@@ -1078,6 +1081,7 @@ __global__ void __launch_bounds__(256) k_s2_dir_scan(const __grid_constant__ S2D
                 lo[k] = min(lo[k], key);
                 hi[k] = max(hi[k], key);
             }
+            if (!MARK) continue;
             int64_t x0, x1, y0, y1;
             xray_point_cells(p, a.has_q ? a.query_from_global : nullptr, a.x0, a.y0, a.edge, a.margin, cells, x0, x1, y0, y1);
             for (int64_t ix = x0; ix <= x1; ++ix)
