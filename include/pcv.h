@@ -354,6 +354,32 @@ int pcv_xray_quadtree_from_dir_filtered_write_dir(pcv_ctx* ctx, const char* octr
                                                   uint32_t nfilt, uint64_t max_device_bytes, const char* out_dir, pcv_xray_quadtree_info* info_out,
                                                   pcv_xray_bounded_info* bounded_info_out, pcv_xray_dir_info* dir_info_out);
 
+/* The X-ray quadtree straight from one or more octree directories (build_xray_quadtree over a list of octree locations), none of
+ * them ever resident as a whole: the same tiles, node set, rect, levels, cancellation and <id>.png + meta<...>.pb outputs as
+ * pcv_xray_quadtree_clouds over pcv_octree_load_dir of every directory, in the same order.  The quadtree lies over the union of
+ * the directories' meta.pb boxes.  XRay tiles are byte for byte the same at every budget and in any order of the directories;
+ * the attribute strategies accumulate as the resident path does.  ndirs = 1 is pcv_xray_quadtree_from_dir_filtered in every
+ * tile, delivery and counter.  One streaming pass over every node's positions of every directory marks the leaves a point falls
+ * into; then each block of leaves runs on one window per directory (each as pcv_xray_quadtree_from_dir selects it), all of a
+ * block's windows on the device together.  The block depth is chosen so that the largest block's windows together fit; nodes the
+ * previous block's window of the same directory holds are copied on the device when the budget holds both blocks' windows.
+ * There is no limit on the total, which may exceed device memory and 2^32 points.  max_device_bytes bounds everything the call
+ * allocates, the windows included (0: most of the free device memory).  pcv_xray_dir_info's counters are summed over the
+ * directories; its largest window is the largest block's windows together.  Errors: ndirs == 0 or a null path ->
+ * PCV_ERR_INVALID; an unreadable meta.pb -> PCV_ERR_IO; a meta.pb other than version 13 -> PCV_ERR_INVALID; a missing or wrongly
+ * sized .xyz / .rgb file -> PCV_ERR_NOT_FOUND, found by stat for every directory before the first read (no tile is delivered);
+ * then the checks of pcv_xray_quadtree_clouds in its order: filters, or an intensity strategy, and a directory without
+ * intensities -> PCV_ERR_INVALID; a binned strategy over more than one directory, or with filters -> PCV_ERR_UNSUPPORTED; a
+ * budget too small for the occupancy pass, a leaf whose windows together do not fit besides one leaf tile (named), a leaf whose
+ * window in one directory holds 2^32 points or more (leaf and directory named) -> PCV_ERR_UNSUPPORTED.  bounded_info_out and
+ * dir_info_out may be NULL. */
+int pcv_xray_quadtree_from_dirs(pcv_ctx* ctx, const char* const* dirs, uint32_t ndirs, const pcv_xray_quadtree_params* params, const pcv_interval* filters,
+                                uint32_t nfilt, uint64_t max_device_bytes, pcv_xray_tile_fn on_tile, void* user, pcv_xray_quadtree_info* info_out,
+                                pcv_xray_bounded_info* bounded_info_out, pcv_xray_dir_info* dir_info_out);
+int pcv_xray_quadtree_from_dirs_write_dir(pcv_ctx* ctx, const char* const* dirs, uint32_t ndirs, const pcv_xray_quadtree_params* params,
+                                          const pcv_interval* filters, uint32_t nfilt, uint64_t max_device_bytes, const char* out_dir,
+                                          pcv_xray_quadtree_info* info_out, pcv_xray_bounded_info* bounded_info_out, pcv_xray_dir_info* dir_info_out);
+
 /* The X-ray quadtree straight from one or more S2 directories (meta.pb + cell files, as pcv_s2_write_dir and pcv_s2_build_to_dir
  * leave them), none of them ever resident as a whole: the same tiles, delivery (every tile after its children; the order across
  * blocks follows the block level, as in every bounded entry), cancellation, <id>.png + meta<...>.pb outputs and

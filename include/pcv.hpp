@@ -744,6 +744,21 @@ pcv_xray_quadtree_info build_xray_quadtree_from_dir(const Context& ctx, const st
                                               &info, bounded_info, dir_info));
     return info;
 }
+// build_xray_quadtree over the octree directories `dirs` streamed from disk, none of them ever resident as a whole: the tiles of
+// build_xray_quadtree over Octrees loaded from each of them, in the same order (pcv_xray_quadtree_from_dirs).
+template <class F>
+pcv_xray_quadtree_info build_xray_quadtree_from_dirs(const Context& ctx, const std::vector<std::string>& dirs, const pcv_xray_quadtree_params& params,
+                                                     const std::vector<ClosedInterval>& filter_intervals, F&& on_tile, uint64_t max_device_bytes = 0,
+                                                     pcv_xray_bounded_info* bounded_info = nullptr, pcv_xray_dir_info* dir_info = nullptr) {
+    std::vector<const char*> raw;
+    for (const std::string& d : dirs) raw.push_back(d.c_str());
+    const std::vector<pcv_interval> f = detail::raw_intervals(filter_intervals);
+    detail::XrayThunk<std::remove_reference_t<F>> th{&on_tile};
+    pcv_xray_quadtree_info info{};
+    check(pcv_xray_quadtree_from_dirs(ctx.raw(), raw.data(), (uint32_t)raw.size(), &params, f.data(), (uint32_t)f.size(), max_device_bytes, &decltype(th)::call,
+                                      &th, &info, bounded_info, dir_info));
+    return info;
+}
 // build_xray_quadtree over the S2 directories `dirs` streamed from disk, none of them ever resident as a whole: the tiles of
 // build_xray_quadtree over S2Cells loaded from each of them, in the same order (pcv_s2_xray_quadtree_from_dirs).
 template <class F>

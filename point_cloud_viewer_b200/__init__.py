@@ -219,6 +219,27 @@ class Context:
         return _xray_call(N.lib().pcv_xray_quadtree_from_dir_filtered_write_dir,
                           (self.h, os.fsencode(str(octree_dir)), C.byref(pr), _p(f), nf, int(max_device_bytes), os.fsencode(str(out_dir))), True)
 
+    def xray_quadtree_from_dirs(self, dirs, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0, query_from_global=None,
+                                background=(255, 255, 255, 255), root=(0, 0), on_tile=None, keep_tiles=True, max_device_bytes=0, filter_intervals=()):
+        """xray_quadtree_clouds over load_dir of every octree directory in `dirs` (one path or a list of paths), streamed from
+        disk window by window, one window per directory and block: the same (info dict, tiles) and keywords, in any total size.
+        One directory is xray_quadtree_from_dir.  `max_device_bytes` bounds everything the call allocates (0: most of the free
+        memory); the info dict also holds the pcv_xray_dir_info fields, summed over the directories."""
+        pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
+        f, nf = _intervals(filter_intervals)
+        arr, keep = _dir_list(dirs)
+        return _xray_call(N.lib().pcv_xray_quadtree_from_dirs, (self.h, arr, len(keep), C.byref(pr), _p(f), nf, int(max_device_bytes)), True, True, on_tile,
+                          keep_tiles)
+
+    def xray_quadtree_from_dirs_write_dir(self, dirs, out_dir, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0,
+                                          query_from_global=None, background=(255, 255, 255, 255), root=(0, 0), max_device_bytes=0, filter_intervals=()):
+        """xray_quadtree_from_dirs with the reference's outputs: <out_dir>/<node id>.png + the quadtree's meta file."""
+        pr = _xray_params(tile_size_px, pixel_size_m, strategy, p0, p1, colormap, bin_size, query_from_global, background, root)
+        f, nf = _intervals(filter_intervals)
+        arr, keep = _dir_list(dirs)
+        return _xray_call(N.lib().pcv_xray_quadtree_from_dirs_write_dir,
+                          (self.h, arr, len(keep), C.byref(pr), _p(f), nf, int(max_device_bytes), os.fsencode(str(out_dir))), True)
+
     # -- X-ray quadtrees straight from S2 directories (never resident as a whole)
     def xray_quadtree_from_s2_dirs(self, dirs, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0, query_from_global=None,
                                    background=(255, 255, 255, 255), root=(0, 0), on_tile=None, keep_tiles=True, max_device_bytes=0, filter_intervals=()):

@@ -247,7 +247,12 @@ SYMBOLS = [
                                                       C.c_void_p, C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo), C.POINTER(XrayDirInfo)]),
     ("pcv_xray_quadtree_from_dir_filtered_write_dir", C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64,
                                                                 C.c_char_p, C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo), C.POINTER(XrayDirInfo)]),
-    ("pcv_xray_quadtree_clouds", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64, XRAY_TILE_FN, C.c_void_p,
+    ("pcv_xray_quadtree_from_dirs", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64,
+                                              XRAY_TILE_FN, C.c_void_p, C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo), C.POINTER(XrayDirInfo)]),
+    ("pcv_xray_quadtree_from_dirs_write_dir", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32,
+                                                        C.c_uint64, C.c_char_p, C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo),
+                                                        C.POINTER(XrayDirInfo)]),
+    ("pcv_xray_quadtree_clouds",C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64, XRAY_TILE_FN, C.c_void_p,
                                            C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo)]),
     ("pcv_xray_quadtree_clouds_write_dir", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64, C.c_char_p,
                                                      C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo)]),

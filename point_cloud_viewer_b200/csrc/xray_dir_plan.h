@@ -5,7 +5,9 @@
 //   octree_children:        the 8 children of every node in that table
 //   xray_window:            the nodes a block of leaves can meet: descend from the octree root while the SAT test is not Out
 //   xray_window_size:       what one window takes in device memory (arrays, query tables, the attribute pass flags)
+//   xray_windows_size:      what the windows of one block over several directories take together
 //   xray_block_location:    a block's location, widened by the pruning margin
+//   xray_occupancy_*:       the occupancy pass's work list of (directory, node) pairs, its device chunk and the chunks
 //   xray_dir_block_depth:   the block depth from the budget, the images and the largest window of the occupied blocks
 #pragma once
 #include <algorithm>
@@ -157,6 +159,74 @@ inline pcv_location xray_block_location(const QuadRect& rect, int B, uint64_t bi
     return xray_location(tmin, tmax, qfg);
 }
 
+// The windows of one block over several directories (windows[k]: directory k's, possibly empty), loaded together: the sum of
+// xray_window_size over the non-empty ones, and the largest one's points and directory (max_dir).
+struct WindowsSize {
+    uint64_t bytes = 0, points = 0, max_points = 0;
+    uint32_t max_dir = 0;
+};
+inline WindowsSize xray_windows_size(const std::vector<const std::vector<pcv_node_meta>*>& tables, const std::vector<char>& has_intensity,
+                                     const std::vector<std::vector<uint32_t>>& windows) {
+    WindowsSize s;
+    for (size_t k = 0; k < windows.size(); ++k) {
+        if (windows[k].empty()) continue;
+        const WindowSize w = xray_window_size(*tables[k], windows[k], has_intensity[k] != 0);
+        s.bytes += w.bytes;
+        s.points += w.points;
+        if (w.points > s.max_points) s.max_points = w.points, s.max_dir = (uint32_t)k;
+    }
+    return s;
+}
+
+// ---- the occupancy pass over the nodes with points of every directory -------------------------------------------------------
+// One node of one of the directories.
+struct DirNode {
+    uint32_t dir, node;
+};
+// The pass's work list: every node with points, directory by directory in list order, each in table order; *largest: the
+// largest node's position bytes.
+inline std::vector<DirNode> xray_occupancy_work(const std::vector<const std::vector<pcv_node_meta>*>& tables, uint64_t* largest) {
+    std::vector<DirNode> work;
+    *largest = 0;
+    for (uint32_t k = 0; k < (uint32_t)tables.size(); ++k)
+        for (uint32_t i = 0; i < (uint32_t)tables[k]->size(); ++i) {
+            const pcv_node_meta& m = (*tables[k])[i];
+            if (m.num_points <= 0) continue;
+            work.push_back(DirNode{k, i});
+            *largest = std::max<uint64_t>(*largest, (uint64_t)m.num_points * 3 * (uint64_t)enc_bytes(m.position_encoding));
+        }
+    return work;
+}
+// Its device chunk: `chunk` position bytes (min(64 MiB, budget / 8), at least the largest node), at most `node_cap` nodes and
+// `tile_cap` work tiles of `tile_points` points; `need`: those arrays (64 B per query node, 16 B per tile) besides `set_bytes`
+// of occupancy set.
+struct OccupancyPlan {
+    uint64_t chunk = 0, node_cap = 0, tile_cap = 0, need = 0;
+};
+inline OccupancyPlan xray_occupancy_plan(uint64_t budget, uint64_t largest, uint32_t tile_points, uint64_t set_bytes) {
+    OccupancyPlan p;
+    p.chunk = std::max<uint64_t>(std::min<uint64_t>(64ull << 20, budget / 8), ((largest + 15) & ~15ull) + 16);
+    p.node_cap = std::max<uint64_t>(64, p.chunk / 512);
+    p.tile_cap = p.node_cap + p.chunk / (3 * (uint64_t)tile_points) + 1;
+    p.need = p.chunk + p.node_cap * 64 + p.tile_cap * 16 + set_bytes;
+    return p;
+}
+// The chunks of the work list: runs of consecutive entries, directories mixed, whose 16-byte aligned positions fit `chunk`
+// and that hold at most node_cap nodes and tile_cap tiles.  The chunk starts plus an end sentinel.
+inline std::vector<size_t> xray_occupancy_chunks(const std::vector<const std::vector<pcv_node_meta>*>& tables, const std::vector<DirNode>& work,
+                                                 const OccupancyPlan& p, uint32_t tile_points) {
+    std::vector<size_t> starts{0};
+    for (size_t k = 0, bytes = 0, nt = 0; k < work.size(); ++k) {
+        const pcv_node_meta& m = (*tables[work[k].dir])[work[k].node];
+        const uint64_t b = ((uint64_t)m.num_points * 3 * (uint64_t)enc_bytes(m.position_encoding) + 15) & ~15ull;
+        const uint64_t t = ((uint64_t)m.num_points + tile_points - 1) / tile_points;
+        if (k > starts.back() && (bytes + b > p.chunk || k - starts.back() >= p.node_cap || nt + t > p.tile_cap)) starts.push_back(k), bytes = 0, nt = 0;
+        bytes += b, nt += t;
+    }
+    starts.push_back(work.size());
+    return starts;
+}
+
 // Block depth g of a directory driver: the largest g <= g_max whose plan `fits(g, w)` holds the block images, the leaf
 // producer's working set and the largest window over the occupied blocks at level deepest - g (`window_max(g)`, UINT64_MAX:
 // a window too large to hold).  A smaller g means a deeper block level and smaller windows.  -1: not even g = 0 fits.
@@ -167,10 +237,13 @@ inline int xray_dir_block_depth(int g_max, const std::function<uint64_t(int)>& w
     }
     return -1;
 }
-// ... for the octree directory: the block images, the node selection and the window fit the budget besides `fixed`.
+// ... for octree directories: the block images, the node selection and the windows fit the budget besides `fixed`; `clouds`
+// directories with points keep their work lists of a key batch at once (xray_pair_bytes).
 inline int xray_dir_block_depth(uint64_t budget, uint64_t fixed, int depth, int g_max, uint64_t leaf_bytes, uint64_t tile_bytes, uint64_t per_loc,
-                                const std::function<uint64_t(int)>& window_max) {
-    return xray_dir_block_depth(g_max, window_max, [&](int g, uint64_t w) { return xray_octree_plan(budget, fixed, w, depth, g, per_loc, leaf_bytes, tile_bytes).g == g; });
+                                const std::function<uint64_t(int)>& window_max, uint32_t clouds = 1) {
+    return xray_dir_block_depth(g_max, window_max, [&](int g, uint64_t w) {
+        return xray_octree_plan(budget, fixed, w, depth, g, per_loc, leaf_bytes, tile_bytes, clouds).g == g;
+    });
 }
 
 }  // namespace pcv
