@@ -380,6 +380,58 @@ int pcv_xray_quadtree_from_dirs_write_dir(pcv_ctx* ctx, const char* const* dirs,
                                           const pcv_interval* filters, uint32_t nfilt, uint64_t max_device_bytes, const char* out_dir,
                                           pcv_xray_quadtree_info* info_out, pcv_xray_bounded_info* bounded_info_out, pcv_xray_dir_info* dir_info_out);
 
+/* merge_xray_quadtrees (xray/src/bin/merge_xray_quadtrees.rs): partial X-ray quadtrees, each written by a *_write_dir entry with
+ * params.root_level / root_index set (<id>.png + meta<digits>.pb), joined into one quadtree in `output_dir`, in the
+ * reference's order:
+ *   1. every input directory must exist (else PCV_ERR_NOT_FOUND) and be a directory (else PCV_ERR_INVALID) (:101-117); the
+ *      output directory is created with its parents if missing (:201-203);
+ *   2. every meta*.pb directly inside each input directory is read (:55-72; subdirectories are not searched), as
+ *      Meta::from_proto reads it (xray/src/lib.rs:59-116): version 3, or version 2 through deprecated_min / _edge_length when
+ *      `min` is unset.  Another version or a malformed file -> PCV_ERR_INVALID naming the file;
+ *   3. validate_and_merge_metadata (:125-176), in its order: no meta file -> PCV_ERR_NOT_FOUND ("No subquadtrees meta files
+ *      found."); every meta empty -> PCV_ERR_INVALID; roots (a meta's node of least level) not unique, roots on different
+ *      levels, deepest_level or tile_size not the same in every meta (empty ones included) -> PCV_ERR_INVALID.  Empty metas are
+ *      skipped and counted.  The merged rect is Node::parent (quadtree/src/lib.rs:100-120) walked to level 0 from the root of
+ *      the first non-empty meta, taking directories in argument order and their meta files by name;
+ *   4. a budget below the walk's device bytes (below) -> PCV_ERR_UNSUPPORTED naming them, before any file is written;
+ *   5. copy_images (:28-46): every *.png directly inside each input directory is copied byte for byte into the output
+ *      directory, except from an input directory that resolves to the output directory;
+ *   6. create_non_leaf_nodes(roots, root level, 0) (generation.rs:656-682, :726-759): every parent from the roots' level - 1 up
+ *      to level 0, build_parent's mosaic of its children (background where one is missing) reduced with Lanczos3 to tile_size,
+ *      as pcv_xray_build_parent makes it, written as <id>.png.  The sub-roots' images are read back from the output
+ *      directory: a missing one -> PCV_ERR_NOT_FOUND; one that is not 8-bit non-interlaced RGBA -> PCV_ERR_UNSUPPORTED; a
+ *      corrupt one or one that is not tile_size px square -> PCV_ERR_INVALID;
+ *   7. meta.pb (version 3): the merged rect, deepest_level, tile_size and every meta's nodes together with the parents.
+ * A call that fails writes no meta.pb, so its output directory does not load as a quadtree.  With root level 0 (one non-empty
+ * meta) nothing is built: the images are copied and meta.pb written.
+ * Device memory: the sub-roots are walked depth-first in index order, each decoded on host threads ahead of the walk and
+ * uploaded once; at most four finished children per level wait for their parent.  The walk holds at most
+ * (4 L + 1) tile_size^2 * 4 bytes of tiles, the vertically reduced mosaic (8 tile_size^2 bytes) and the Lanczos3 taps
+ * (device_bytes_needed); max_device_bytes bounds it (0: most of the free device memory).  Parent tiles are encoded and written
+ * by the PNG writer threads of pcv_xray_quadtree_bounded_write_dir.  Null pointers -> PCV_ERR_INVALID; a file that cannot be
+ * read, listed, copied or written -> PCV_ERR_IO. */
+typedef struct pcv_xray_merge_info {
+    uint32_t metas_read;          /* meta*.pb files read                                                          */
+    uint32_t metas_empty;         /* of those, the ones without nodes (skipped)                                   */
+    uint8_t root_level;           /* level of the sub-roots                                                       */
+    uint8_t deepest_level;        /* Meta::deepest_level                                                          */
+    uint32_t tile_size_px;        /* Meta::tile_size                                                              */
+    uint64_t roots_decoded;       /* sub-root PNGs decoded and uploaded                                           */
+    uint64_t parents_built;       /* parent tiles built and written                                               */
+    uint64_t files_copied;        /* *.png files copied into the output directory                                 */
+    uint64_t bytes_copied;
+    float ms_parents;             /* CUDA events: the parents' Lanczos3 kernels                                   */
+    double ms_copy;               /* wall time of the copy                                                        */
+    double ms_decode;             /* wall time of reading and decoding the sub-root PNGs, summed over them        */
+    double ms_write;              /* wall time of encoding and writing the parent PNGs, summed over them          */
+    double ms_total;              /* wall time of the whole call                                                  */
+    uint64_t max_device_bytes;    /* the budget used                                                              */
+    uint64_t device_bytes_needed; /* what the walk may hold at most                                               */
+    uint64_t peak_device_bytes;   /* the most the walk held at once                                               */
+} pcv_xray_merge_info;
+int pcv_xray_merge_quadtrees(pcv_ctx* ctx, const char* const* input_dirs, uint32_t n, const char* output_dir, const uint8_t background[4],
+                             uint64_t max_device_bytes, pcv_xray_merge_info* info_out);
+
 /* The X-ray quadtree straight from one or more S2 directories (meta.pb + cell files, as pcv_s2_write_dir and pcv_s2_build_to_dir
  * leave them), none of them ever resident as a whole: the same tiles, delivery (every tile after its children; the order across
  * blocks follows the block level, as in every bounded entry), cancellation, <id>.png + meta<...>.pb outputs and

@@ -759,6 +759,15 @@ pcv_xray_quadtree_info build_xray_quadtree_from_dirs(const Context& ctx, const s
                                       &th, &info, bounded_info, dir_info));
     return info;
 }
+// merge_xray_quadtrees: the sub-root builds in `input_dirs` joined into one quadtree in `output_dir` (pcv_xray_merge_quadtrees).
+inline pcv_xray_merge_info merge_xray_quadtrees(const Context& ctx, const std::vector<std::string>& input_dirs, const std::string& output_dir,
+                                                const std::array<uint8_t, 4>& background = {255, 255, 255, 255}, uint64_t max_device_bytes = 0) {
+    std::vector<const char*> raw;
+    for (const std::string& d : input_dirs) raw.push_back(d.c_str());
+    pcv_xray_merge_info info{};
+    check(pcv_xray_merge_quadtrees(ctx.raw(), raw.data(), (uint32_t)raw.size(), output_dir.c_str(), background.data(), max_device_bytes, &info));
+    return info;
+}
 // build_xray_quadtree over the S2 directories `dirs` streamed from disk, none of them ever resident as a whole: the tiles of
 // build_xray_quadtree over S2Cells loaded from each of them, in the same order (pcv_s2_xray_quadtree_from_dirs).
 template <class F>

@@ -51,6 +51,7 @@ def device_count():
 
 
 XRAY_COLORED, XRAY_INTENSITY, XRAY_HEIGHT_STDDEV = 1, 2, 3
+WHITE, TRANSPARENT = (255, 255, 255, 255), (255, 255, 255, 0)  # tile_background_color (xray/src/generation.rs:44-56)
 
 
 class Context:
@@ -239,6 +240,18 @@ class Context:
         arr, keep = _dir_list(dirs)
         return _xray_call(N.lib().pcv_xray_quadtree_from_dirs_write_dir,
                           (self.h, arr, len(keep), C.byref(pr), _p(f), nf, int(max_device_bytes), os.fsencode(str(out_dir))), True)
+
+    # -- merging partial X-ray quadtrees
+    def merge_xray_quadtrees(self, input_dirs, output_dir, background=WHITE, max_device_bytes=0):
+        """merge_xray_quadtrees (pcv_xray_merge_quadtrees): the sub-root builds in `input_dirs` (one path or a list of paths; each
+        holds <id>.png + meta<digits>.pb files of one or more sub-roots at one level) joined into one quadtree in `output_dir`:
+        their images copied, the levels above the sub-roots built on the GPU, meta.pb written.  `max_device_bytes` bounds the
+        device memory of the parents' walk (0: most of the free memory).  Returns the pcv_xray_merge_info fields as a dict."""
+        arr, keep = _dir_list(input_dirs)
+        info = N.XrayMergeInfo()
+        bg = (C.c_uint8 * 4)(*background)
+        N.check(N.lib().pcv_xray_merge_quadtrees(self.h, arr, len(keep), os.fsencode(str(output_dir)), bg, int(max_device_bytes), C.byref(info)))
+        return {f: getattr(info, f) for f, _ in N.XrayMergeInfo._fields_}
 
     # -- X-ray quadtrees straight from S2 directories (never resident as a whole)
     def xray_quadtree_from_s2_dirs(self, dirs, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0, query_from_global=None,

@@ -144,6 +144,15 @@ class XrayDirInfo(C.Structure):
                 ("largest_window_points", C.c_uint64), ("occupied_leaves", C.c_uint64), ("ms_occupancy", C.c_double), ("ms_windows", C.c_double)]
 
 
+class XrayMergeInfo(C.Structure):
+    """pcv_xray_merge_info (include/pcv.h)."""
+
+    _fields_ = [("metas_read", C.c_uint32), ("metas_empty", C.c_uint32), ("root_level", C.c_uint8), ("deepest_level", C.c_uint8),
+                ("tile_size_px", C.c_uint32), ("roots_decoded", C.c_uint64), ("parents_built", C.c_uint64), ("files_copied", C.c_uint64),
+                ("bytes_copied", C.c_uint64), ("ms_parents", C.c_float), ("ms_copy", C.c_double), ("ms_decode", C.c_double), ("ms_write", C.c_double),
+                ("ms_total", C.c_double), ("max_device_bytes", C.c_uint64), ("device_bytes_needed", C.c_uint64), ("peak_device_bytes", C.c_uint64)]
+
+
 class DirQueryStats(C.Structure):
     """pcv_dir_query_stats (include/pcv.h)."""
 
@@ -252,6 +261,7 @@ SYMBOLS = [
     ("pcv_xray_quadtree_from_dirs_write_dir", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32,
                                                         C.c_uint64, C.c_char_p, C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo),
                                                         C.POINTER(XrayDirInfo)]),
+    ("pcv_xray_merge_quadtrees", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_char_p, C.c_void_p, C.c_uint64, C.POINTER(XrayMergeInfo)]),
     ("pcv_xray_quadtree_clouds",C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64, XRAY_TILE_FN, C.c_void_p,
                                            C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo)]),
     ("pcv_xray_quadtree_clouds_write_dir", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64, C.c_char_p,

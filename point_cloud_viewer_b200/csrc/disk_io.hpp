@@ -86,6 +86,16 @@ struct Cursor {
         p += 8;
         return d;
     }
+    float fixed32() {
+        if (end - p < 4) {
+            bad = true;
+            return 0;
+        }
+        float f;
+        memcpy(&f, p, 4);
+        p += 4;
+        return f;
+    }
     Cursor sub() {
         uint64_t n = varint();
         if ((uint64_t)(end - p) < n) {
