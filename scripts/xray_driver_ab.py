@@ -1,6 +1,7 @@
 """A/B of two builds of the library on the bounded X-ray quadtree driver, e.g. a build of the parent commit against the tree's
-own: every source (resident octree, octree directory, S2 cloud) on the seeded scenes of its GPU tests, at the smallest and the
-default budgets those tests use, all four strategies with and without query_from_global, a sub-root, a run cancelled from
+own: every source (resident octree, octree directory, several octree directories, S2 cloud, one or several S2 directories) on the
+seeded scenes of its GPU tests, at the smallest and the default budgets those tests use and, for the directory lists, budgets
+that make the windows reuse the previous block's nodes, all four strategies with and without query_from_global, a sub-root, a run cancelled from
 on_tile, budgets too small to run and write_dir.  Each library runs in its own process.  Every tile is hashed as it is
 delivered, so the two runs must agree on every tile's bytes and on the delivery order; they must also agree on every field of
 the info dict except the ms_* timings, on every error's code and message, and on every file write_dir writes.  Library A runs
@@ -158,6 +159,105 @@ def s2_cases(pcv, out):
     ctx.close()
 
 
+def dirs_common(pcv, out, name, run, run_dir, T, px, qfg, filters):
+    """The cases every list of directories runs: a budget scan, the strategies, a sub-root, filters, cancels, a budget too small
+    and write_dir.  run(T, px, **kw) / run_dir(out_dir, T, px, **kw) call the entry over the scene's directories."""
+    import numpy as np
+
+    for b in [int(v) for v in np.geomspace(256 << 10, 48 << 20, 12)] + [0]:
+        out["%s/scan/%d" % (name, b)] = record(run, T, px, query_from_global=qfg, max_device_bytes=b)
+    for sname, kw in strategies(pcv).items():
+        for budget in (3 << 20, 0):
+            out["%s/%s/%d" % (name, sname, budget)] = record(run, T, px, background=TRANSPARENT, max_device_bytes=budget, **kw)
+    for budget in (3 << 20, 0):
+        out["%s/subroot/%d" % (name, budget)] = record(run, T, px, query_from_global=qfg, root=(1, 2), max_device_bytes=budget)
+        out["%s/filters/%d" % (name, budget)] = record(run, T, px, filter_intervals=filters, max_device_bytes=budget)
+    for k in (1, 5, 40):
+        out["%s/cancel/%d" % (name, k)] = record(run, T, px, cancel_after=k, max_device_bytes=3 << 20)
+    out["%s/too_small" % name] = record(run, T, px, max_device_bytes=64 << 10)
+    for budget in (3 << 20, 0):
+        out["%s/write_dir/%d" % (name, budget)] = record_dir(run_dir, T, px, query_from_global=qfg, max_device_bytes=budget)
+
+
+def octree_dirs_cases(pcv, out, tmp):
+    """test_zzf_xray_octree_dirs_gpu.py's four directories: two overlapping parts of the slab at 4000 and 1500 points per node,
+    clusters beside it written by build_octree_to_dir at 2500, and a part of the slab without intensities."""
+    import numpy as np
+
+    n = 150_000
+    x, y, z, rgb = pcv.synth_points_host(pcv.SYNTH_SLAB_ECEF, 80293751232, 0, n)
+    xyz = np.stack([x, y, z], 1)
+    rgb = np.asarray(rgb).reshape(-1, 3)
+    inten = ((np.arange(n) * 7919) % 1000).astype(np.float32)
+    _, _, res = pcv.synth_bbox(pcv.SYNTH_SLAB_ECEF)
+    m = 40_000
+    cx, cy, cz, crgb = pcv.synth_points_host(pcv.SYNTH_GAUSS_CLUSTERS, 7, 0, m)
+    c = np.stack([cx, cy, cz], 1)
+    c = (c - c.min(0)) / np.ptp(c, 0).max()
+    ext = xyz.max(0) - xyz.min(0)
+    cxyz = xyz.max(0) + np.array([0.05, -0.3, -0.5]) * ext + c * 0.4 * ext
+    cinten = ((np.arange(m) * 31) % 1000).astype(np.float32)
+    col = lambda p, k: np.ascontiguousarray(p[:, k])  # noqa: E731
+    dirs = [os.path.join(tmp, "dirs_" + name) for name in ("a", "b", "c", "bare")]
+    for d, (lo, hi), mppn, with_i in ((dirs[0], (0, 90_000), 4000, True), (dirs[1], (60_000, n), 1500, True), (dirs[3], (20_000, 70_000), 4000, False)):
+        bc = pcv.Context(0, max_points_per_node=mppn)
+        p = xyz[lo:hi]
+        t = bc.build_octree(col(p, 0), col(p, 1), col(p, 2), rgb[lo:hi].reshape(-1).copy(), res, p.min(0), p.max(0),
+                            intensity=inten[lo:hi].copy() if with_i else None)
+        t.write_dir(d)
+        t.free()
+        bc.close()
+    bc = pcv.Context(0, max_points_per_node=2500)
+    bc.build_octree_to_dir(dirs[2], col(cxyz, 0), col(cxyz, 1), col(cxyz, 2), np.asarray(crgb).reshape(-1).copy(), res, cxyz.min(0), cxyz.max(0),
+                           intensity=cinten, max_points_in_core=15_000)
+    bc.close()
+    ctx = pcv.Context(0)
+    hs = [ctx.open_dir(d) for d in dirs[:3]]
+    box = np.concatenate([np.min([h.bbox_min for h in hs], 0), np.max([h.bbox_max for h in hs], 0)])
+    for h in hs:
+        h.close()
+    T = 32
+    px = float(max(box[3] - box[0], box[4] - box[1])) / (T * 2 ** 5)
+    for name, ds in (("dirs3", dirs[:3]), ("dirs4", dirs), ("dirs4_permuted", [dirs[k] for k in (3, 1, 0, 2)])):
+        run = lambda *a, ds=ds, **kw: ctx.xray_quadtree_from_dirs(ds, *a, **kw)  # noqa: E731
+        run_dir = lambda o, *a, ds=ds, **kw: ctx.xray_quadtree_from_dirs_write_dir(ds, o, *a, **kw)  # noqa: E731
+        if name == "dirs4":  # intensity strategies and filters are refused with the directory without intensities
+            out["%s/scan/0" % name] = record(run, T, px, query_from_global=slab_qfg(pcv), max_device_bytes=0)
+            out["%s/scan/small" % name] = record(run, T, px, query_from_global=slab_qfg(pcv), max_device_bytes=3 << 20)
+            out["%s/filters" % name] = record(run, T, px, filter_intervals=[(100.0, 600.0)])
+            continue
+        dirs_common(pcv, out, name, run, run_dir, T, px, slab_qfg(pcv), [(100.0, 600.0), (700.0, 800.0)])
+    ctx.close()
+
+
+def s2_dirs_cases(pcv, out, tmp):
+    """test_zzc_s2_dir_xray_gpu.py's scene: the 1e6-point slab written with build_s2_dir at level 20, as one directory and as
+    three overlapping parts."""
+    import numpy as np
+
+    ctx = pcv.Context(0)
+    n = 1_000_000
+    x, y, z, rgb = pcv.synth_points_host(pcv.SYNTH_SLAB_ECEF, 80293751232, 0, n)
+    rgb = np.asarray(rgb).reshape(-1, 3)
+    inten = np.random.default_rng(3).uniform(0.0, 100.0, n).astype(np.float32)
+    one = os.path.join(tmp, "s2_l20")
+    ctx.build_s2_dir(one, x, y, z, rgb.reshape(-1).copy(), inten, split_level=20)
+    parts = []
+    for k, (a, b) in enumerate([(0, int(0.45 * n)), (int(0.3 * n), int(0.75 * n)), (int(0.6 * n), n)]):
+        parts.append(os.path.join(tmp, "s2_part%d" % k))
+        ctx.build_s2_dir(parts[-1], x[a:b].copy(), y[a:b].copy(), z[a:b].copy(), rgb[a:b].reshape(-1).copy(), inten[a:b].copy(), split_level=20)
+    h = ctx.open_s2_dir(one)
+    ext = h.bbox_max - h.bbox_min
+    h.close()
+    T = 64
+    px = float(max(ext[0], ext[1])) / (T * 32)
+    for name, ds in (("s2dir", [one]), ("s2dirs3", parts), ("s2dirs3_permuted", parts[::-1])):
+        run = lambda *a, ds=ds, **kw: ctx.xray_quadtree_from_s2_dirs(ds, *a, **kw)  # noqa: E731
+        run_dir = lambda o, *a, ds=ds, **kw: ctx.xray_quadtree_from_s2_dirs_write_dir(ds, o, *a, **kw)  # noqa: E731
+        dirs_common(pcv, out, name, run, run_dir, T, px, slab_qfg(pcv), [(10.0, 60.0), (70.0, 80.0)])
+    ctx.close()
+
+
 def child(path):
     sys.path.insert(0, ROOT)
     import point_cloud_viewer_b200 as pcv
@@ -165,9 +265,29 @@ def child(path):
     out = {}
     with tempfile.TemporaryDirectory() as tmp:
         octree_cases(pcv, out, tmp)
+        octree_dirs_cases(pcv, out, tmp)
+        s2_dirs_cases(pcv, out, tmp)
     s2_cases(pcv, out)
     with open(path, "wb") as f:
         pickle.dump(out, f)
+
+
+def what_differs(x, y):
+    """The parts of two records of one case that differ: the info fields (with both values), the tile bytes, the delivery order,
+    the files, the error."""
+    if not x or not y:
+        return dict(missing="a" if not x else "b")
+    out = {}
+    xi, yi = x.get("info") or {}, y.get("info") or {}
+    out.update({"info." + k: (xi.get(k), yi.get(k)) for k in sorted(set(xi) | set(yi)) if xi.get(k) != yi.get(k)})
+    if [t[:2] for t in x.get("order", ())] != [t[:2] for t in y.get("order", ())]:
+        out["order"] = True
+    elif x.get("order") != y.get("order"):
+        out["tile_bytes"] = True
+    for k in ("files", "error"):
+        if x.get(k) != y.get(k):
+            out[k] = (str(x.get(k))[:200], str(y.get(k))[:200])
+    return out
 
 
 def main():
@@ -198,8 +318,8 @@ def main():
     res = dict(cases=len(keys), equal=len(equal), unstable_in_a=len(unstable), unstable_equal_but_bytes=len(unstable) - len(set(unstable) & set(differ)),
                errors=sum("error" in v for v in a.values()), tiles=sum(len(v.get("order", v.get("files", ()))) for v in a.values()),
                unstable=unstable[:30], differ=differ[:20])
-    for k in differ[:5]:
-        res["diff/" + k] = dict(a=str(a.get(k))[:400], b=str(b.get(k))[:400])
+    for k in differ[:40]:
+        res["diff/" + k] = what_differs(a.get(k), b.get(k))
     print(json.dumps(res))
     if args.out:
         with open(args.out, "w") as f:
