@@ -432,6 +432,57 @@ typedef struct pcv_xray_merge_info {
 int pcv_xray_merge_quadtrees(pcv_ctx* ctx, const char* const* input_dirs, uint32_t n, const char* output_dir, const uint8_t background[4],
                              uint64_t max_device_bytes, pcv_xray_merge_info* info_out);
 
+/* inpaint_xray_quadtree (xray/src/bin/inpaint_xray_quadtree.rs, xray/src/inpaint.rs): the leaves of the (possibly partial)
+ * quadtree with root R = (root_level, root_index) in `input_dir` - meta<R>.pb and <id>.png files as the *_write_dir entries
+ * and pcv_xray_merge_quadtrees leave them, built with a transparent background - get their small holes filled, into
+ * `output_dir` (created if missing; it may be `input_dir`):
+ *   1. meta<R>.pb is read (missing -> PCV_ERR_NOT_FOUND, as is a missing input directory); the leaves are its nodes at
+ *      deepest_level.  A leaf outside R, or R outside its level -> PCV_ERR_INVALID; an odd tile size -> PCV_ERR_UNSUPPORTED;
+ *   2. the adjacent leaves (:41-71): the deepest nodes of the metas of R's Left, Top, Right and Bottom neighbour pieces in
+ *      `input_dir` whose neighbour in the opposite direction is a leaf (a warning on stderr when there is none and R is not
+ *      the root);
+ *   3. with inpaint_distance_px = k > 0, every leaf gets a 2T x 2T image stitched from the visible tiles of its 3 x 3
+ *      neighbourhood (transparent (255, 255, 255, 0) elsewhere).  Visible: in place (the same realpath) every <id>.png of
+ *      deepest_level in the directory; otherwise the leaves and the adjacent leaves.  The alpha channel is closed (dilate,
+ *      then erode, LInf square of radius k, clipped to the image); a closed pixel of alpha 0 takes the RGBA of the nearest
+ *      pixel of alpha != 0 in Euclidean distance, the smaller column, then the smaller row on a tie (texture synthesis in the
+ *      reference: see DESIGN.md section 3).  Each image is blended with its Right, then its Bottom neighbour's where that
+ *      neighbour is a leaf (weights i / (T - 1), rounded per channel, in f32), and the centre T x T is kept;
+ *   4. every leaf's pixels of alpha < 128 become `background` (assign_background_color); k = 0 does only this;
+ *   5. the parents from deepest_level - 1 up to root_level, as pcv_xray_merge_quadtrees builds them, from the leaves;
+ *   6. the adjacent leaves are not left in `output_dir`, and (copying) meta<R>.pb is copied last, so that a failed call
+ *      leaves no meta there.
+ * A listed leaf (copying: or adjacent leaf) that is missing or cannot be read -> PCV_ERR_IO; one that is not T x T px ->
+ * PCV_ERR_INVALID; k > 255 -> PCV_ERR_INVALID.  Device memory: the leaves go in aligned 2^j x 2^j blocks in index order, j the
+ * largest (at most 5) whose block and the parents' walk fit max_device_bytes (0: most of the free device memory); a budget
+ * below device_bytes_needed (j = 0) -> PCV_ERR_UNSUPPORTED naming it, before any file is written.  The output does not depend
+ * on the budget.  Null pointers -> PCV_ERR_INVALID. */
+typedef struct pcv_xray_inpaint_info {
+    uint8_t root_level;
+    uint8_t deepest_level;
+    uint32_t tile_size_px;
+    uint32_t inpaint_distance_px;
+    uint32_t block_depth;         /* j: blocks of 2^j x 2^j leaves                                               */
+    uint64_t leaves;              /* the meta's nodes at deepest_level                                           */
+    uint64_t adjacent_leaves;     /* leaves of the neighbour pieces next to them                                 */
+    uint64_t tiles_decoded;       /* PNGs decoded (halo tiles count once per block that reads them)              */
+    uint64_t hole_pixels_filled;  /* over the leaves' inpaint images, each counted once                          */
+    uint64_t blocks;
+    uint64_t parents_built;
+    uint64_t files_copied;        /* meta<R>.pb when copying                                                     */
+    uint64_t bytes_copied;
+    uint64_t max_device_bytes;    /* the budget used                                                             */
+    uint64_t device_bytes_needed; /* what blocks of one leaf and the parents' walk hold at most                  */
+    uint64_t peak_device_bytes;   /* the most held at once                                                       */
+    double ms_decode;             /* wall time of reading and decoding the tiles, summed over them               */
+    double ms_kernels;            /* CUDA events: stitch, close, fill, blends, crop and background               */
+    double ms_parents;            /* CUDA events: the parents' Lanczos3 kernels                                  */
+    double ms_encode;             /* wall time of encoding and writing the PNGs, summed over them                */
+    double ms_total;              /* wall time of the whole call                                                 */
+} pcv_xray_inpaint_info;
+int pcv_xray_inpaint_quadtree(pcv_ctx* ctx, const char* input_dir, const char* output_dir, uint8_t root_level, uint64_t root_index,
+                              uint32_t inpaint_distance_px, const uint8_t background[4], uint64_t max_device_bytes, pcv_xray_inpaint_info* info_out);
+
 /* The X-ray quadtree straight from one or more S2 directories (meta.pb + cell files, as pcv_s2_write_dir and pcv_s2_build_to_dir
  * leave them), none of them ever resident as a whole: the same tiles, delivery (every tile after its children; the order across
  * blocks follows the block level, as in every bounded entry), cancellation, <id>.png + meta<...>.pb outputs and

@@ -768,6 +768,16 @@ inline pcv_xray_merge_info merge_xray_quadtrees(const Context& ctx, const std::v
     check(pcv_xray_merge_quadtrees(ctx.raw(), raw.data(), (uint32_t)raw.size(), output_dir.c_str(), background.data(), max_device_bytes, &info));
     return info;
 }
+// inpaint_xray_quadtree: the leaves of the quadtree with root (root_level, root_index) in `input_dir` inpainted into
+// `output_dir`, their background assigned and the parents rebuilt (pcv_xray_inpaint_quadtree).
+inline pcv_xray_inpaint_info inpaint_xray_quadtree(const Context& ctx, const std::string& input_dir, const std::string& output_dir, uint32_t inpaint_distance_px,
+                                                   const std::array<uint8_t, 4>& background = {255, 255, 255, 255}, uint8_t root_level = 0,
+                                                   uint64_t root_index = 0, uint64_t max_device_bytes = 0) {
+    pcv_xray_inpaint_info info{};
+    check(pcv_xray_inpaint_quadtree(ctx.raw(), input_dir.c_str(), output_dir.c_str(), root_level, root_index, inpaint_distance_px, background.data(),
+                                    max_device_bytes, &info));
+    return info;
+}
 // build_xray_quadtree over the S2 directories `dirs` streamed from disk, none of them ever resident as a whole: the tiles of
 // build_xray_quadtree over S2Cells loaded from each of them, in the same order (pcv_s2_xray_quadtree_from_dirs).
 template <class F>

@@ -253,6 +253,19 @@ class Context:
         N.check(N.lib().pcv_xray_merge_quadtrees(self.h, arr, len(keep), os.fsencode(str(output_dir)), bg, int(max_device_bytes), C.byref(info)))
         return {f: getattr(info, f) for f, _ in N.XrayMergeInfo._fields_}
 
+    # -- inpainting an X-ray quadtree
+    def inpaint_xray_quadtree(self, input_dir, output_dir, inpaint_distance_px, background=WHITE, root=(0, 0), max_device_bytes=0):
+        """inpaint_xray_quadtree (pcv_xray_inpaint_quadtree): the leaves of the quadtree with root `root` = (level, index) in
+        `input_dir`, built with a transparent background, get their holes of radius up to `inpaint_distance_px` (0..255) filled
+        across tile borders on the GPU; then their pixels of alpha < 128 become `background` and the parents are rebuilt, into
+        `output_dir` (which may be `input_dir`).  `max_device_bytes` bounds the device memory (0: most of the free memory); the
+        output does not depend on it.  Returns the pcv_xray_inpaint_info fields as a dict."""
+        info = N.XrayInpaintInfo()
+        bg = (C.c_uint8 * 4)(*background)
+        N.check(N.lib().pcv_xray_inpaint_quadtree(self.h, os.fsencode(str(input_dir)), os.fsencode(str(output_dir)), int(root[0]), int(root[1]),
+                                                  int(inpaint_distance_px), bg, int(max_device_bytes), C.byref(info)))
+        return {f: getattr(info, f) for f, _ in N.XrayInpaintInfo._fields_}
+
     # -- X-ray quadtrees straight from S2 directories (never resident as a whole)
     def xray_quadtree_from_s2_dirs(self, dirs, tile_size_px, pixel_size_m, strategy=0, p0=0.0, p1=0.0, colormap=0, bin_size=0.0, query_from_global=None,
                                    background=(255, 255, 255, 255), root=(0, 0), on_tile=None, keep_tiles=True, max_device_bytes=0, filter_intervals=()):

@@ -153,6 +153,15 @@ class XrayMergeInfo(C.Structure):
                 ("ms_total", C.c_double), ("max_device_bytes", C.c_uint64), ("device_bytes_needed", C.c_uint64), ("peak_device_bytes", C.c_uint64)]
 
 
+class XrayInpaintInfo(C.Structure):
+    """pcv_xray_inpaint_info (include/pcv.h)."""
+
+    _fields_ = [("root_level", C.c_uint8), ("deepest_level", C.c_uint8), ("tile_size_px", C.c_uint32), ("inpaint_distance_px", C.c_uint32),
+                ("block_depth", C.c_uint32), ("leaves", C.c_uint64), ("adjacent_leaves", C.c_uint64), ("tiles_decoded", C.c_uint64),
+                ("hole_pixels_filled", C.c_uint64), ("blocks", C.c_uint64), ("parents_built", C.c_uint64), ("files_copied", C.c_uint64),
+                ("bytes_copied", C.c_uint64), ("max_device_bytes", C.c_uint64), ("device_bytes_needed", C.c_uint64), ("peak_device_bytes", C.c_uint64),
+                ("ms_decode", C.c_double), ("ms_kernels", C.c_double), ("ms_parents", C.c_double), ("ms_encode", C.c_double), ("ms_total", C.c_double)]
+
 class DirQueryStats(C.Structure):
     """pcv_dir_query_stats (include/pcv.h)."""
 
@@ -262,6 +271,8 @@ SYMBOLS = [
                                                         C.c_uint64, C.c_char_p, C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo),
                                                         C.POINTER(XrayDirInfo)]),
     ("pcv_xray_merge_quadtrees", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_char_p, C.c_void_p, C.c_uint64, C.POINTER(XrayMergeInfo)]),
+    ("pcv_xray_inpaint_quadtree", C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_uint8, C.c_uint64, C.c_uint32, C.c_void_p, C.c_uint64,
+                                            C.POINTER(XrayInpaintInfo)]),
     ("pcv_xray_quadtree_clouds",C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64, XRAY_TILE_FN, C.c_void_p,
                                            C.POINTER(XrayQuadtreeInfo), C.POINTER(XrayBoundedInfo)]),
     ("pcv_xray_quadtree_clouds_write_dir", C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64, C.c_char_p,

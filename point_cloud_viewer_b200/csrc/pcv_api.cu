@@ -572,6 +572,7 @@ int pcv_synth_bbox(int kind, double bbox_min[3], double bbox_max[3], double* res
 #include "query_api.inl"
 #include "xray_api.inl"
 #include "xray_merge.inl"
+#include "xray_inpaint.inl"
 #include "dir_octree.inl"
 #include "xray_dir.inl"
 #include "dir_query.inl"
