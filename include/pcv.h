@@ -196,6 +196,23 @@ int pcv_query_cell_union(const pcv_octree* o, const pcv_cell_union* cu, const pc
 int pcv_query_cell_unions_batch_device(const pcv_octree* o, const pcv_cell_union* unions, uint32_t nunion, const pcv_interval* filters,
                                        uint32_t nfilt, uint64_t* counts_out, uint64_t* tested_out);
 
+/* Batched queries that return their points.  For locations L0..Ln-1 the call fills the host offsets offsets_out[0..n] and writes,
+ * for every i, the points pcv_query_points(Li) (pcv_query_cell_union for a union) streams, in the same order and bit for bit in
+ * every field, to [offsets_out[i], offsets_out[i+1]) of the device arrays d_xyz (3 f64 per point), d_rgb (3 u8), d_intensity
+ * (f32) and d_src (u64, the build input index).  offsets_out[i+1] - offsets_out[i] is pcv_query_batch_device's counts_out[i]; a
+ * location's segment does not depend on the other locations of the call.
+ * d_xyz == NULL is a size query: offsets_out is filled and nothing is written.  d_rgb, d_intensity and d_src may each be NULL to
+ * skip the field; a non-null d_intensity on points without intensity (or a non-null d_rgb on an S2 cloud without colour) is
+ * PCV_ERR_INVALID.  cap < offsets_out[n] is PCV_ERR_INVALID with offsets_out complete (the device arrays are then unspecified).
+ * The argument contract of pcv_query_points holds; a selection too large for one call is PCV_ERR_UNSUPPORTED ("split the
+ * batch").  pcv_last_query_stats: returned_points = offsets_out[n], stored_points = the points written, tested_points as
+ * pcv_query_batch_device; ms_select covers selection and ordering, ms_cull the count, scan and place passes. */
+int pcv_query_batch_points_device(const pcv_octree* o, const pcv_location* locs, uint32_t nloc, const pcv_interval* filters, uint32_t nfilt,
+                                  uint64_t* offsets_out, double* d_xyz, uint8_t* d_rgb, float* d_intensity, uint64_t* d_src, uint64_t cap);
+int pcv_query_cell_unions_batch_points_device(const pcv_octree* o, const pcv_cell_union* unions, uint32_t nunion, const pcv_interval* filters,
+                                              uint32_t nfilt, uint64_t* offsets_out, double* d_xyz, uint8_t* d_rgb, float* d_intensity,
+                                              uint64_t* d_src, uint64_t cap);
+
 /* Timing / traffic of the last pcv_query_batch_device call on the context (CUDA events on the context's stream). */
 typedef struct pcv_query_stats {
     float ms_device;            /* first kernel to last kernel of the call                                   */
@@ -621,6 +638,13 @@ int pcv_s2_query_batch_device(const pcv_s2cloud* cloud, const pcv_location* locs
                               uint32_t nfilt, uint64_t* counts_out, uint64_t* tested_out);
 int pcv_s2_query_cell_unions_batch_device(const pcv_s2cloud* cloud, const pcv_cell_union* unions, uint32_t nunion,
                                           const pcv_interval* filters, uint32_t nfilt, uint64_t* counts_out, uint64_t* tested_out);
+/* pcv_query_batch_points_device over the cloud: each segment is what pcv_s2_query_points / pcv_s2_query_cell_union streams. */
+int pcv_s2_query_batch_points_device(const pcv_s2cloud* cloud, const pcv_location* locs, uint32_t nloc, const pcv_interval* filters,
+                                     uint32_t nfilt, uint64_t* offsets_out, double* d_xyz, uint8_t* d_rgb, float* d_intensity, uint64_t* d_src,
+                                     uint64_t cap);
+int pcv_s2_query_cell_unions_batch_points_device(const pcv_s2cloud* cloud, const pcv_cell_union* unions, uint32_t nunion,
+                                                 const pcv_interval* filters, uint32_t nfilt, uint64_t* offsets_out, double* d_xyz, uint8_t* d_rgb,
+                                                 float* d_intensity, uint64_t* d_src, uint64_t cap);
 /* The directory an S2Splitter<RawNodeWriter> leaves behind (read_write/s2.rs:127-145, raw.rs): per cell `<to_token()>.xyz`
  * (f64 LE x, y, z), `.rgb`, `.intensity`, and meta.pb = Meta { version 13, bounding_box, s2 { cells, attributes } }
  * (s2_cells/mod.rs:77-104); load = S2Cells::from_data_provider over such a directory (:106-147, :203-216; versions < 12 and

@@ -175,6 +175,17 @@ inline std::vector<pcv_cell_union> raw_unions(const std::vector<CellUnion>& us) 
     for (auto& u : us) raw.push_back(raw_union(u));
     return raw;
 }
+// A pcv_*_batch_points_device entry over raw locations or cell unions: offsets (one per location, plus one) on the host, the
+// points to the device arrays.  Returns the total.
+template <class Fn, class H, class Raw>
+uint64_t batch_points(Fn fn, H h, const std::vector<Raw>& raw, const std::vector<ClosedInterval>& filter_intervals, std::vector<uint64_t>& offsets,
+                      double* d_xyz, uint8_t* d_rgb, float* d_intensity, uint64_t* d_src, uint64_t cap) {
+    std::vector<pcv_interval> f;
+    for (auto& iv : filter_intervals) f.push_back(pcv_interval{iv.lower_bound, iv.upper_bound});
+    offsets.assign(raw.size() + 1, 0);
+    check(fn(h, raw.data(), (uint32_t)raw.size(), f.empty() ? nullptr : f.data(), (uint32_t)f.size(), offsets.data(), d_xyz, d_rgb, d_intensity, d_src, cap));
+    return offsets.back();
+}
 }  // namespace detail
 
 struct NodeData {  // octree/mod.rs:147-152
@@ -232,6 +243,22 @@ class Octree {
         counts.assign(unions.size(), 0);
         tested.assign(unions.size(), 0);
         check(pcv_query_cell_unions_batch_device(o_, raw.data(), (uint32_t)raw.size(), nullptr, 0, counts.data(), tested.data()));
+    }
+    // The points of every location in device memory (pcv_query_batch_points_device): [offsets[i], offsets[i + 1]) of the device
+    // arrays, which hold cap points, is what for_each_batch streams for locs[i].  d_xyz == nullptr: offsets only; d_rgb,
+    // d_intensity and d_src may be nullptr.  Returns the total.
+    uint64_t query_batch_points(const std::vector<PointLocation>& locs, const std::vector<ClosedInterval>& filter_intervals, std::vector<uint64_t>& offsets,
+                                double* d_xyz = nullptr, uint8_t* d_rgb = nullptr, float* d_intensity = nullptr, uint64_t* d_src = nullptr,
+                                uint64_t cap = 0) const {
+        std::vector<pcv_location> raw;
+        for (auto& l : locs) raw.push_back(l.raw);
+        return detail::batch_points(pcv_query_batch_points_device, o_, raw, filter_intervals, offsets, d_xyz, d_rgb, d_intensity, d_src, cap);
+    }
+    uint64_t query_batch_points(const std::vector<CellUnion>& unions, const std::vector<ClosedInterval>& filter_intervals, std::vector<uint64_t>& offsets,
+                                double* d_xyz = nullptr, uint8_t* d_rgb = nullptr, float* d_intensity = nullptr, uint64_t* d_src = nullptr,
+                                uint64_t cap = 0) const {
+        return detail::batch_points(pcv_query_cell_unions_batch_points_device, o_, detail::raw_unions(unions), filter_intervals, offsets, d_xyz, d_rgb,
+                                    d_intensity, d_src, cap);
     }
     NodeData get_node_data(const NodeId& id) const {  // mod.rs:285-307
         for (auto& m : nodes_)
@@ -618,6 +645,20 @@ class S2Cells {
         counts.assign(unions.size(), 0);
         tested.assign(unions.size(), 0);
         check(pcv_s2_query_cell_unions_batch_device(s_, raw.data(), (uint32_t)raw.size(), nullptr, 0, counts.data(), tested.data()));
+    }
+    // Octree::query_batch_points over the cloud (pcv_s2_query_batch_points_device)
+    uint64_t query_batch_points(const std::vector<PointLocation>& locs, const std::vector<ClosedInterval>& filter_intervals, std::vector<uint64_t>& offsets,
+                                double* d_xyz = nullptr, uint8_t* d_rgb = nullptr, float* d_intensity = nullptr, uint64_t* d_src = nullptr,
+                                uint64_t cap = 0) const {
+        std::vector<pcv_location> raw;
+        for (auto& l : locs) raw.push_back(l.raw);
+        return detail::batch_points(pcv_s2_query_batch_points_device, s_, raw, filter_intervals, offsets, d_xyz, d_rgb, d_intensity, d_src, cap);
+    }
+    uint64_t query_batch_points(const std::vector<CellUnion>& unions, const std::vector<ClosedInterval>& filter_intervals, std::vector<uint64_t>& offsets,
+                                double* d_xyz = nullptr, uint8_t* d_rgb = nullptr, float* d_intensity = nullptr, uint64_t* d_src = nullptr,
+                                uint64_t cap = 0) const {
+        return detail::batch_points(pcv_s2_query_cell_unions_batch_points_device, s_, detail::raw_unions(unions), filter_intervals, offsets, d_xyz, d_rgb,
+                                    d_intensity, d_src, cap);
     }
     // build_xray_quadtree (xray/src/build_quadtree.rs) over the cloud, with the leaf queries' filter intervals: every tile through
     // `on_tile` in post-order, as Octree::build_xray_quadtree delivers it.  `max_device_bytes` bounds the call's device memory.

@@ -698,6 +698,14 @@ class Octree:
         """(counts, tested) per location; the locations are all pcv_locations or all geometry.CellUnions."""
         return _query_batch(N.lib().pcv_query_batch_device, N.lib().pcv_query_cell_unions_batch_device, self.h, locs, filters)
 
+    def query_batch_points(self, locs, filters=(), fields=None):
+        """The points of every location, in device memory: (offsets, {field: torch CUDA tensor}).  offsets (uint64, len(locs) + 1)
+        cut the tensors into one segment per location, in order; segment i holds exactly what query_points(locs[i], filters=filters)
+        streams, in the same order.  fields: any of "xyz" (n, 3) f64, "rgb" (n, 3) u8, "intensity" (n,) f32 and "src" (n,) int64;
+        None: every field the octree holds.  The locations are all pcv_locations or all geometry.CellUnions."""
+        return _query_batch_points(N.lib().pcv_query_batch_points_device, N.lib().pcv_query_cell_unions_batch_points_device, self, locs, filters, fields,
+                                   True, self.has_intensity)
+
     def last_query_stats(self):
         """Timing / traffic of the last query_batch_device call (pcv_query_stats)."""
         st = N.QueryStats()
@@ -796,6 +804,47 @@ def _query_points(fn, h, loc, callback, filters, batch_size):
         raise PcvError(rc, "cancelled by callback")
     N.check(rc)
     return got
+
+
+BATCH_POINT_FIELDS = {"xyz": (3, "<f8"), "rgb": (3, "|u1"), "intensity": (None, "<f4"), "src": (None, "<i8")}
+
+
+def _query_batch_points(fn, fn_union, cloud, locs, filters, fields, has_rgb, has_intensity):
+    """Octree / S2Cloud.query_batch_points: the size query, one DeviceBuffer per field, then the call that fills them."""
+    import torch
+
+    if fields is None:
+        fields = [k for k, ok in (("xyz", True), ("rgb", has_rgb), ("intensity", has_intensity), ("src", True)) if ok]
+    fields = list(dict.fromkeys(fields))
+    for k in fields:
+        if k not in BATCH_POINT_FIELDS:
+            raise ValueError("unknown field %r (fields: %s)" % (k, ", ".join(BATCH_POINT_FIELDS)))
+    arr, fn = _batch_locations(fn, fn_union, locs)
+    f = np.asarray(filters, np.float64).reshape(-1)
+    nf = len(f) // 2
+    off = np.zeros(len(locs) + 1, np.uint64)
+    N.check(fn(cloud.h, arr, len(locs), _p(f) if nf else None, nf, _p(off), None, None, None, None, 0))
+    total = int(off[-1])
+    shape = lambda k: (total,) if BATCH_POINT_FIELDS[k][0] is None else (total, BATCH_POINT_FIELDS[k][0])
+    if total == 0:
+        dtypes = {"<f8": torch.float64, "|u1": torch.uint8, "<f4": torch.float32, "<i8": torch.int64}
+        return off, {k: torch.empty(shape(k), dtype=dtypes[BATCH_POINT_FIELDS[k][1]], device=torch.device("cuda", cloud.ctx.device)) for k in fields}
+    bufs = {k: cloud.ctx.device_buffer(shape(k), BATCH_POINT_FIELDS[k][1]) for k in fields}
+    if "xyz" not in bufs:  # the positions are always written: a buffer the caller does not get
+        bufs["xyz"] = cloud.ctx.device_buffer(shape("xyz"), "<f8")
+    ptr = lambda k: bufs[k].ptr if k in bufs else None
+    N.check(fn(cloud.h, arr, len(locs), _p(f) if nf else None, nf, _p(off), ptr("xyz"), ptr("rgb"), ptr("intensity"), ptr("src"), total))
+    return off, {k: bufs[k].tensor() for k in fields}
+
+
+def _batch_locations(fn, fn_union, locs):
+    """The C array of a batch of locations and the entry that takes it: all pcv_locations (fn) or all geometry.CellUnions (fn_union)."""
+    unions = [isinstance(loc, geometry.CellUnion) for loc in locs]
+    if any(unions):
+        if not all(unions):
+            raise ValueError("a batch of locations holds cell unions and other locations; query them in separate batches")
+        return (N.CellUnion * len(locs))(*[loc.struct() for loc in locs]), fn_union
+    return (N.Location * len(locs))(*locs), fn
 
 
 def _query_batch(fn, fn_union, h, locs, filters):
@@ -972,6 +1021,12 @@ class S2Cloud:
     def query_batch_device(self, locs, filters=()):
         """(counts, tested) per location, as Octree.query_batch_device; the locations are all pcv_locations or all geometry.CellUnions."""
         return _query_batch(N.lib().pcv_s2_query_batch_device, N.lib().pcv_s2_query_cell_unions_batch_device, self.h, locs, filters)
+
+    def query_batch_points(self, locs, filters=(), fields=None):
+        """Octree.query_batch_points over the cloud: segment i holds what query_points(locs[i], filters=filters) streams.  fields
+        None: every field the cloud holds ("rgb" only with colour, "intensity" only with intensity)."""
+        return _query_batch_points(N.lib().pcv_s2_query_batch_points_device, N.lib().pcv_s2_query_cell_unions_batch_points_device, self, locs, filters,
+                                   fields, self.has_color, self.has_intensity)
 
     def last_query_stats(self):
         """Timing / traffic of the last query_batch_device call on the context (pcv_query_stats)."""

@@ -244,6 +244,8 @@ SYMBOLS = [
     ("pcv_nodes_in_cell_union", C.c_int, [C.c_void_p, C.POINTER(CellUnion), C.c_void_p, C.c_uint64, _u64p]),
     ("pcv_query_cell_union", C.c_int, [C.c_void_p, C.POINTER(CellUnion), C.c_void_p, C.c_uint32, C.c_uint64, BATCH_CB, C.c_void_p]),
     ("pcv_query_cell_unions_batch_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
+    ("pcv_query_batch_points_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]),
+    ("pcv_query_cell_unions_batch_points_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]),
     ("pcv_last_query_stats", C.c_int, [C.c_void_p, C.POINTER(QueryStats)]),
     ("pcv_last_xray_stats", C.c_int, [C.c_void_p, C.POINTER(XrayStats)]),
     ("pcv_xray_tile", C.c_int, [C.c_void_p, _dp, _dp, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]),
@@ -305,6 +307,8 @@ SYMBOLS = [
     ("pcv_s2_query_cell_union", C.c_int, [C.c_void_p, C.POINTER(CellUnion), C.c_void_p, C.c_uint32, C.c_uint64, BATCH_CB, C.c_void_p]),
     ("pcv_s2_query_batch_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
     ("pcv_s2_query_cell_unions_batch_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
+    ("pcv_s2_query_batch_points_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]),
+    ("pcv_s2_query_cell_unions_batch_points_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]),
     ("pcv_s2_write_dir", C.c_int, [C.c_void_p, C.c_char_p]),
     ("pcv_s2_load_dir", C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),
     ("pcv_s2_dir_open", C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, C.POINTER(C.c_void_p)]),

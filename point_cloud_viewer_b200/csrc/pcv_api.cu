@@ -577,6 +577,7 @@ int pcv_synth_bbox(int kind, double bbox_min[3], double bbox_max[3], double* res
 #include "xray_dir.inl"
 #include "dir_query.inl"
 #include "s2_api.inl"
+#include "query_batch_points.inl"
 #include "s2_xray.inl"
 #include "s2_dir_xray.inl"
 #include "s2_dir_query.inl"
