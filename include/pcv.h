@@ -585,6 +585,26 @@ typedef struct pcv_dir_query_stats {  /* the last call on the handle            
     uint32_t kernel_launches;
 } pcv_dir_query_stats;
 int pcv_octree_dir_last_stats(const pcv_octree_dir* d, pcv_dir_query_stats* out);
+/* pcv_query_batch_points_device over the directory: [offsets_out[i], offsets_out[i+1]) of the device arrays holds what
+ * pcv_octree_dir_query_points (pcv_octree_dir_query_cell_union for a union) streams for Li, in the same order and bit for bit
+ * (d_src: the slot), and offsets_out[i+1] - offsets_out[i] is pcv_octree_dir_query_batch's counts_out[i].  The size query, NULL
+ * fields and the argument checks are the resident entry's.  Two passes over one chunk list: a count pass reads every visited
+ * node once (.xyz, and .intensity with filters); unless this is a size query, a place pass reads the nodes again (.xyz, and
+ * .rgb / .intensity for the fields written or the filters) and writes every survivor at its position; the chunk the count
+ * pass ended on is placed without a second read, so a batch whose visited nodes fit one chunk reads every file once.
+ * cap < offsets_out[n] is PCV_ERR_INVALID naming both numbers, with offsets_out complete, decided before the place pass: the
+ * device arrays are untouched.  max_device_bytes bounds everything but the caller's arrays; a batch whose frontier or per-tile
+ * state (4 bytes per (location, node tile)) does not fit -> PCV_ERR_UNSUPPORTED ("split the batch"), the handle still usable.
+ * A node file rewritten between the passes -> PCV_ERR_IO (no write ever goes past a tile's counted survivors or past cap).
+ * pcv_octree_dir_last_stats: returned_points = offsets_out[n]; tested_points and visited_pairs as query_batch; chunks,
+ * node_files_read, bytes_read, bytes_uploaded and ms_cull over both passes (bytes_uploaded counts every chunk image whole,
+ * including the colour / intensity regions a count-pass chunk carries for the place pass without reading them). */
+int pcv_octree_dir_query_batch_points_device(const pcv_octree_dir* d, const pcv_location* locs, uint32_t nloc, const pcv_interval* filters,
+                                             uint32_t nfilt, uint64_t* offsets_out, double* d_xyz, uint8_t* d_rgb, float* d_intensity,
+                                             uint64_t* d_src, uint64_t cap);
+int pcv_octree_dir_query_cell_unions_batch_points_device(const pcv_octree_dir* d, const pcv_cell_union* unions, uint32_t nunion,
+                                                         const pcv_interval* filters, uint32_t nfilt, uint64_t* offsets_out, double* d_xyz,
+                                                         uint8_t* d_rgb, float* d_intensity, uint64_t* d_src, uint64_t cap);
 
 /* ---- f4: the S2-cell point cloud (src/read_write/s2.rs, src/s2_cells/mod.rs, src/geometry/s2_cell_union.rs) ---- */
 /* Cell ids are the S2 library's 64-bit CellID values (face, Hilbert position, level marker bit); the arithmetic is the `s2`
@@ -752,6 +772,13 @@ int pcv_s2_dir_query_batch(const pcv_s2_dir* d, const pcv_location* locs, uint32
 int pcv_s2_dir_query_cell_unions_batch(const pcv_s2_dir* d, const pcv_cell_union* unions, uint32_t nunion, const pcv_interval* filters,
                                        uint32_t nfilt, uint64_t* counts_out, uint64_t* tested_out);
 int pcv_s2_dir_last_stats(const pcv_s2_dir* d, pcv_dir_query_stats* out);
+/* pcv_octree_dir_query_batch_points_device over the cells: each segment is what pcv_s2_dir_query_points /
+ * pcv_s2_dir_query_cell_union streams (d_src: the slot); a non-null d_rgb on a directory without colour is PCV_ERR_INVALID. */
+int pcv_s2_dir_query_batch_points_device(const pcv_s2_dir* d, const pcv_location* locs, uint32_t nloc, const pcv_interval* filters, uint32_t nfilt,
+                                         uint64_t* offsets_out, double* d_xyz, uint8_t* d_rgb, float* d_intensity, uint64_t* d_src, uint64_t cap);
+int pcv_s2_dir_query_cell_unions_batch_points_device(const pcv_s2_dir* d, const pcv_cell_union* unions, uint32_t nunion, const pcv_interval* filters,
+                                                     uint32_t nfilt, uint64_t* offsets_out, double* d_xyz, uint8_t* d_rgb, float* d_intensity,
+                                                     uint64_t* d_src, uint64_t cap);
 /* CellUnion::contains for arbitrary points: mask_out[i] = union.contains_cellid(CellID::from_point(p_i)). */
 int pcv_s2_union_contains(pcv_ctx* ctx, const pcv_points* host_points, const uint64_t* union_ids, uint32_t n_union, uint8_t* mask_out);
 

@@ -439,6 +439,21 @@ class OctreeDir {
         tested.assign(unions.size(), 0);
         check(pcv_octree_dir_query_cell_unions_batch(d_, raw.data(), (uint32_t)raw.size(), nullptr, 0, counts.data(), tested.data()));
     }
+    // Octree::query_batch_points over the directory (pcv_octree_dir_query_batch_points_device): [offsets[i], offsets[i + 1]) of the
+    // device arrays is what for_each_batch streams for locs[i] (source_index = slot).  Returns the total.
+    uint64_t query_batch_points(const std::vector<PointLocation>& locs, const std::vector<ClosedInterval>& filter_intervals, std::vector<uint64_t>& offsets,
+                                double* d_xyz = nullptr, uint8_t* d_rgb = nullptr, float* d_intensity = nullptr, uint64_t* d_src = nullptr,
+                                uint64_t cap = 0) const {
+        std::vector<pcv_location> raw;
+        for (auto& l : locs) raw.push_back(l.raw);
+        return detail::batch_points(pcv_octree_dir_query_batch_points_device, d_, raw, filter_intervals, offsets, d_xyz, d_rgb, d_intensity, d_src, cap);
+    }
+    uint64_t query_batch_points(const std::vector<CellUnion>& unions, const std::vector<ClosedInterval>& filter_intervals, std::vector<uint64_t>& offsets,
+                                double* d_xyz = nullptr, uint8_t* d_rgb = nullptr, float* d_intensity = nullptr, uint64_t* d_src = nullptr,
+                                uint64_t cap = 0) const {
+        return detail::batch_points(pcv_octree_dir_query_cell_unions_batch_points_device, d_, detail::raw_unions(unions), filter_intervals, offsets, d_xyz,
+                                    d_rgb, d_intensity, d_src, cap);
+    }
     std::vector<uint8_t> nodes_data_blob(const std::vector<NodeId>& ids) const {
         std::vector<uint64_t> hl;
         for (auto& id : ids) hl.push_back(id.high), hl.push_back(id.low);
@@ -731,6 +746,20 @@ class S2CellsDir {
         counts.assign(unions.size(), 0);
         tested.assign(unions.size(), 0);
         check(pcv_s2_dir_query_cell_unions_batch(d_, raw.data(), (uint32_t)raw.size(), nullptr, 0, counts.data(), tested.data()));
+    }
+    // Octree::query_batch_points over the directory's cells (pcv_s2_dir_query_batch_points_device; source_index = slot)
+    uint64_t query_batch_points(const std::vector<PointLocation>& locs, const std::vector<ClosedInterval>& filter_intervals, std::vector<uint64_t>& offsets,
+                                double* d_xyz = nullptr, uint8_t* d_rgb = nullptr, float* d_intensity = nullptr, uint64_t* d_src = nullptr,
+                                uint64_t cap = 0) const {
+        std::vector<pcv_location> raw;
+        for (auto& l : locs) raw.push_back(l.raw);
+        return detail::batch_points(pcv_s2_dir_query_batch_points_device, d_, raw, filter_intervals, offsets, d_xyz, d_rgb, d_intensity, d_src, cap);
+    }
+    uint64_t query_batch_points(const std::vector<CellUnion>& unions, const std::vector<ClosedInterval>& filter_intervals, std::vector<uint64_t>& offsets,
+                                double* d_xyz = nullptr, uint8_t* d_rgb = nullptr, float* d_intensity = nullptr, uint64_t* d_src = nullptr,
+                                uint64_t cap = 0) const {
+        return detail::batch_points(pcv_s2_dir_query_cell_unions_batch_points_device, d_, detail::raw_unions(unions), filter_intervals, offsets, d_xyz, d_rgb,
+                                    d_intensity, d_src, cap);
     }
     pcv_dir_query_stats last_stats() const {
         pcv_dir_query_stats st{};

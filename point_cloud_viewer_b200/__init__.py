@@ -810,7 +810,7 @@ BATCH_POINT_FIELDS = {"xyz": (3, "<f8"), "rgb": (3, "|u1"), "intensity": (None, 
 
 
 def _query_batch_points(fn, fn_union, cloud, locs, filters, fields, has_rgb, has_intensity):
-    """Octree / S2Cloud.query_batch_points: the size query, one DeviceBuffer per field, then the call that fills them."""
+    """Octree / S2Cloud / OctreeDir / S2Dir.query_batch_points: the size query, one DeviceBuffer per field, then the call that fills them."""
     import torch
 
     if fields is None:
@@ -918,6 +918,13 @@ class OctreeDir:
     def query_batch(self, locs, filters=()):
         """(counts, tested) of Octree.query_batch_device, every visited node read once."""
         return _query_batch(N.lib().pcv_octree_dir_query_batch, N.lib().pcv_octree_dir_query_cell_unions_batch, self.h, locs, filters)
+
+    def query_batch_points(self, locs, filters=(), fields=None):
+        """Octree.query_batch_points over the directory: (offsets, {field: torch CUDA tensor}), segment i holding what
+        query_points(locs[i], filters=filters) streams (src: the slot).  A size query counts first, so the visited nodes'
+        positions are read once more than by the C entry given large enough arrays; last_stats() describes the second call."""
+        return _query_batch_points(N.lib().pcv_octree_dir_query_batch_points_device, N.lib().pcv_octree_dir_query_cell_unions_batch_points_device, self,
+                                   locs, filters, fields, True, self.has_intensity)
 
     def nodes_data_blob(self, names, out=None):
         ids = np.zeros(2 * len(names), np.uint64)
@@ -1121,6 +1128,11 @@ class S2Dir:
     def query_batch(self, locs, filters=()):
         """(counts, tested) of S2Cloud.query_batch_device, every selected cell read once."""
         return _query_batch(N.lib().pcv_s2_dir_query_batch, N.lib().pcv_s2_dir_query_cell_unions_batch, self.h, locs, filters)
+
+    def query_batch_points(self, locs, filters=(), fields=None):
+        """S2Cloud.query_batch_points over the directory (src: the slot); the size query as in OctreeDir.query_batch_points."""
+        return _query_batch_points(N.lib().pcv_s2_dir_query_batch_points_device, N.lib().pcv_s2_dir_query_cell_unions_batch_points_device, self, locs,
+                                   filters, fields, self.has_color, self.has_intensity)
 
     def last_stats(self):
         """pcv_dir_query_stats of the last call on the handle ("node" counters count cells)."""

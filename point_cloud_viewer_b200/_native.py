@@ -292,6 +292,8 @@ SYMBOLS = [
     ("pcv_octree_dir_query_cell_unions_batch", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
     ("pcv_octree_dir_nodes_data_blob", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, _u64p]),
     ("pcv_octree_dir_last_stats", C.c_int, [C.c_void_p, C.POINTER(DirQueryStats)]),
+    ("pcv_octree_dir_query_batch_points_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]),
+    ("pcv_octree_dir_query_cell_unions_batch_points_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]),
     ("pcv_s2_cell_ids", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_uint32, C.c_void_p]),
     ("pcv_s2_build", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_uint32, C.POINTER(C.c_void_p)]),
     ("pcv_s2_build_device", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_uint32, C.POINTER(C.c_void_p)]),
@@ -323,6 +325,8 @@ SYMBOLS = [
     ("pcv_s2_dir_query_batch", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
     ("pcv_s2_dir_query_cell_unions_batch", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]),
     ("pcv_s2_dir_last_stats", C.c_int, [C.c_void_p, C.POINTER(DirQueryStats)]),
+    ("pcv_s2_dir_query_batch_points_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]),
+    ("pcv_s2_dir_query_cell_unions_batch_points_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]),
     ("pcv_s2_build_to_dir", C.c_int, [C.c_void_p, C.POINTER(Points), C.c_uint32, C.c_uint64, C.c_char_p, C.POINTER(S2DirBuildInfo)]),
     ("pcv_s2_build_from_file_to_dir", C.c_int, [C.c_void_p, C.c_char_p, C.c_uint32, C.c_uint64, C.c_char_p, C.POINTER(S2DirBuildInfo)]),
     ("pcv_s2_xray_quadtree", C.c_int, [C.c_void_p, C.POINTER(XrayQuadtreeParams), C.c_void_p, C.c_uint32, C.c_uint64, XRAY_TILE_FN, C.c_void_p,

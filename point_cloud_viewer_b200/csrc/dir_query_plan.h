@@ -2,6 +2,7 @@
 // compile it with g++).
 //   dir_chunk_bytes:  what one chunk takes in device memory (inputs, chunk-local tables, survivors)
 //   plan_dir_chunks:  the visited nodes, in visit order, cut into chunks of pieces at kDirTile boundaries under a byte bound
+//   dir_chunk_tiles:  the work tiles of one chunk, in the order its tile table lists them
 //   nodes_blob_layout / nodes_blob_header: the /nodes_data reply of pcv_nodes_data_blob, laid out from the node table alone
 #pragma once
 #include <algorithm>
@@ -52,16 +53,17 @@ inline uint64_t dir_chunk_bytes(uint64_t points, uint64_t xyz_bytes, uint64_t pi
 // The smallest chunk any query needs: one tile at the widest encoding, with its survivors.
 inline uint64_t dir_min_chunk_bytes() { return dir_chunk_bytes(kDirTile, (uint64_t)kDirTile * 24, 1, 1, true, true); }
 
-// Cuts the visited nodes (in visit order) into chunks whose dir_chunk_bytes stays within `chunk_budget`.  Each piece takes as
-// many whole tiles of its node as fit (the node's last tile may be short), so a node larger than a chunk is split across
-// consecutive chunks.  False: a single tile of some node does not fit an empty chunk.
+// Cuts the visited nodes (in visit order) into chunks whose dir_chunk_bytes, plus `tile_bytes` more per work tile, stays within
+// `chunk_budget`.  Each piece takes as many whole tiles of its node as fit (the node's last tile may be short), so a node larger
+// than a chunk is split across consecutive chunks.  False: a single tile of some node does not fit an empty chunk.
 inline bool plan_dir_chunks(const std::vector<uint32_t>& visit, const std::function<DirPlanNode(uint32_t)>& info, bool has_i, bool store,
-                            uint64_t chunk_budget, std::vector<DirChunk>& out) {
+                            uint64_t chunk_budget, std::vector<DirChunk>& out, uint64_t tile_bytes = 0) {
     out.clear();
     DirChunk cur;
     auto cost_with = [&](const DirChunk& c, const DirPlanNode& d, uint64_t cnt) {
         const uint64_t tiles = (cnt + kDirTile - 1) / kDirTile * d.mult;
-        return dir_chunk_bytes(c.points + cnt, c.xyz_bytes + dir_align(cnt * 3 * d.bpc, 16), c.pieces.size() + 1, c.tiles + tiles, has_i, store);
+        return dir_chunk_bytes(c.points + cnt, c.xyz_bytes + dir_align(cnt * 3 * d.bpc, 16), c.pieces.size() + 1, c.tiles + tiles, has_i, store) +
+               (tile_bytes ? dir_align(tile_bytes * (c.tiles + tiles), kDirAlign) : 0);
     };
     for (uint32_t v : visit) {
         const DirPlanNode d = info(v);
@@ -92,6 +94,22 @@ inline bool plan_dir_chunks(const std::vector<uint32_t>& visit, const std::funct
     }
     if (!cur.pieces.empty()) out.push_back(std::move(cur));
     return true;
+}
+
+// The work tiles of chunk `ch`, in the order of its tile table: per piece k, per location that visits the piece's node - the run
+// [(*pair_begin)[node], (*pair_begin)[node + 1]) of *pair_loc (batched form), or the one location (*node_flag)[node] (0 without
+// flags) - the piece's tiles in file order.  f(k, location, first point of the tile inside the piece, points of the tile).
+template <class F>
+inline void dir_chunk_tiles(const DirChunk& ch, const std::vector<uint32_t>* pair_loc, const std::vector<uint64_t>* pair_begin,
+                            const std::vector<uint32_t>* node_flag, F&& f) {
+    for (size_t k = 0; k < ch.pieces.size(); ++k) {
+        const DirPiece& pc = ch.pieces[k];
+        const uint64_t lb = pair_begin ? (*pair_begin)[pc.node] : 0, le = pair_begin ? (*pair_begin)[pc.node + 1] : 1;
+        const uint32_t loc0 = node_flag ? (*node_flag)[pc.node] : 0u;
+        for (uint64_t j = lb; j < le; ++j)
+            for (uint64_t t = 0; t < pc.count; t += kDirTile)
+                f((uint32_t)k, pair_loc ? (*pair_loc)[j] : loc0, (uint32_t)t, (uint32_t)std::min<uint64_t>(kDirTile, pc.count - t));
+    }
 }
 
 // ---- /nodes_data reply (octree_web_viewer/src/backend.rs:66-75 pad, :92-165 get_nodes_data), from the node table ----------

@@ -581,6 +581,7 @@ int pcv_synth_bbox(int kind, double bbox_min[3], double bbox_max[3], double* res
 #include "s2_xray.inl"
 #include "s2_dir_xray.inl"
 #include "s2_dir_query.inl"
+#include "dir_query_batch_points.inl"
 #include "ply_api.inl"
 #include "shard_api.inl"
 #include "sharded_build.inl"
